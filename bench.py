@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the hot path (BASELINE.json metric), one JSON line on stdout (rank 0).
 
-  python bench.py --gpus N --steps K --warmup W            # B200-native arm, 3DGS rasterizer (configs 1 / 2)
+  python bench.py --gpus N --steps K --warmup W            # CUDA arm (H100, sm_90a), 3DGS rasterizer (configs 1 / 2)
   python bench.py --impl reference --steps K --warmup W    # CPU arm: the pure-PyTorch oracle port
   python bench.py --workload ngp   [--impl reference]      # BASELINE config 3 (Instant-NGP), single GPU
   python bench.py --workload mesh  [--impl reference]      # BASELINE config 4 (mesh ops), single GPU
@@ -14,8 +14,13 @@ cloud (1M Gaussians D0, SH degree 3, 1920x1080), gradients summed over views in 
           --ar-chunks > 1 cuts it into Gaussian-range chunks behind the last pass: measured, does not pay, DESIGN.md 7);
           the weak-scaling figure with 8 views per rank is measured too and reported as config.weak_8_views_per_rank.
 metric = Msplats/s = N_gaussians * (views of all ranks) / t.
+
+--dump-outputs DIR writes what the timed step computed in its last timed step as DIR/<name>.npy (float32 / float64,
+at most 64 MiB in all; larger outputs as a fixed, seeded row sample), so that two builds can be compared output for
+output: the inputs are seeded, so the same arguments give the same inputs on every run.
 """
 import argparse
+import atexit
 import json
 import math
 import os
@@ -50,7 +55,38 @@ def parse():
     ap.add_argument("--cpu-sample", default="50000,480,270")
     ap.add_argument("--ar-chunks", type=int, default=1, help="Gaussian-range chunks of the overlapped all-reduce")
     ap.add_argument("--triangles", type=int, default=500_000, help="mesh workload: triangle count")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (CUDA arm, rank 0)")
     return ap.parse_args()
+
+
+DUMP_LIMIT = 64 * 2 ** 20
+DUMP_ROWS = 200_000          # Gaussians sampled from the packed gradient buffer (62 floats each at SH degree 3)
+
+
+def dump_outputs(out_dir, arrays):
+    """arrays: name -> tensor / array; floating arrays keep float64 or become float32, integer arrays become float64.
+    When they exceed DUMP_LIMIT, every array over 1 MiB is cut to a fixed, seeded sample of its rows (last axis = one
+    row), written as <name>.npy with the sampled row numbers in <name>_rows.npy."""
+    import numpy as np
+    import torch
+    conv = {}
+    for name, a in arrays.items():
+        a = a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)
+        conv[name] = np.ascontiguousarray(a, dtype=np.float64 if a.dtype in (np.float64, np.int64, np.int32) else np.float32)
+    total = sum(a.nbytes for a in conv.values())
+    if total > DUMP_LIMIT:
+        large = [k for k, a in conv.items() if a.nbytes > 2 ** 20]
+        small = total - sum(conv[k].nbytes for k in large)
+        rows = {k: conv[k].reshape(-1, conv[k].shape[-1] if conv[k].ndim > 1 else 1) for k in large}
+        frac = (0.95 * DUMP_LIMIT - small) / sum(r.shape[0] * (r.itemsize * r.shape[1] + 8) for r in rows.values())
+        rng = np.random.default_rng(0)
+        for k, r in rows.items():
+            idx = np.sort(rng.choice(r.shape[0], max(1, int(r.shape[0] * frac)), replace=False))
+            conv[k], conv[k + "_rows"] = r[idx], idx.astype(np.float64)
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in conv.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def peaks():
@@ -60,7 +96,7 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:  # noqa: BLE001
             pass
-    return 6650.0, "fallback 6.65 TB/s"
+    return 3350.0, "H100 SXM data sheet 3.35 TB/s"
 
 
 def traffic_of(kernel):
@@ -88,6 +124,14 @@ class Clocks:
                                        "-i", str(gpu_index), "-lms", str(int(interval_ms))], stdout=self.f, stderr=subprocess.DEVNULL)
         except Exception:  # noqa: BLE001
             self.p = None
+        atexit.register(self._end)        # the poller must not outlive bench.py when a measurement raises
+
+    def _end(self):
+        if self.p is not None and self.p.poll() is None:
+            self.p.kill()
+            self.p.wait()
+        if os.path.exists(self.f.name):
+            os.unlink(self.f.name)
 
     def stop(self):
         out = {"sm_mhz": None, "sm_max_mhz": None, "reasons": []}
@@ -258,6 +302,16 @@ def run_gs(args):
     clocks = Clocks(local, 20 if world == 1 else 100) if rank == 0 else None
     main = measure(V, args.steps, max(args.warmup, 3))
     clk = clocks.stop() if clocks else None
+    if args.dump_outputs and rank == 0:
+        # the packed gradient buffer of the last timed step (all-reduced when world > 1), sampled at fixed Gaussians
+        rows = torch.randperm(N, generator=torch.Generator().manual_seed(0))[:min(N, DUMP_ROWS)].sort().values
+        ri = rows.to(dev)
+        arrays = {"gaussian_index": rows, "pairs": torch.tensor([main["pairs"]], dtype=torch.int64)}
+        o = 0
+        for nm, wdt in zip(("means3D", "shs", "opacities", "scales", "rotations", "means2D"), parallel.GROUP_WIDTHS(M)):
+            arrays["grad_" + nm] = params.grads[o:o + N * wdt].view(N, wdt).index_select(0, ri)
+            o += N * wdt
+        dump_outputs(args.dump_outputs, arrays)
     ms_step, value, launches = main["ms_step"], main["value"], main["launches"]
     weak = None
     if world > 1 and V != 8:
@@ -358,7 +412,7 @@ def run_gs(args):
                            + (f"config 1: {V}-view orbit (radius 1.75, fovy 49.1)" if world == 1 else
                               f"config 2: 200-view orbit ring dealt over {world} ranks, {V} views per rank per step")),
               "views_per_gpu": V, "gaussians": N, "pairs_per_view": pairs_view, "pairs_per_view_after_tile_culling": pairs_proc,
-              "l2": "inputs larger than L2 (236 MB parameters + views x 41 MB upstream gradients per step vs 126 MB L2); no flush needed",
+              "l2": "inputs larger than L2 (236 MB parameters + views x 41 MB upstream gradients per step vs 50 MB L2); no flush needed",
               "parallelism": f"views sharded over {world} rank(s), Gaussians replicated" + (
                   f", one NCCL all-reduce of the 248 MB packed gradient buffer per step, issued from inside the step in "
                   f"{args.ar_chunks} Gaussian-range chunk(s) (gs_b200_set_grad_sink)" if world > 1 else "")}
@@ -458,7 +512,8 @@ def run_ngp(args):
     x, y, z = torch.meshgrid(g, g, g, indexing="ij")
     est.binaries = ((x * x + y * y + z * z) < 0.25)[None]; est.occs = est.binaries.flatten().float()
     fovy = 49.1
-    params = list(enc_d.parameters()) + list(enc_c.parameters()) + list(mlp_d.parameters()) + list(mlp_c.parameters())
+    modules = {"enc_d": enc_d, "enc_c": enc_c, "mlp_d": mlp_d, "mlp_c": mlp_c}
+    params = [q for mod in modules.values() for q in mod.parameters()]
 
     def rays_of(pose):        # InstantNGP.get_rays (Instant_NGP.py:37-70)
         xs_, ys_ = torch.meshgrid(torch.arange(W, device=dev), torch.arange(H, device=dev), indexing="xy")
@@ -490,9 +545,11 @@ def run_ngp(args):
         loss = (img * target).sum()
         loss.backward()
         enc_d.grad_total_variation(1e-8)
+        st["grads"] = {f"grad_{m}_{n}".replace(".", "_"): q.grad for m, mod in modules.items()
+                      for n, q in mod.named_parameters() if q.grad is not None}
         for q in params:
             q.grad = None
-        st["samples"], st["p"] = ri.numel(), p.detach()
+        st["samples"], st["p"], st["img"], st["loss"] = ri.numel(), p.detach(), img.detach(), loss.detach()
         return img, loss
 
     def step():
@@ -510,6 +567,9 @@ def run_ngp(args):
     clocks = Clocks(0)
     ms_step = timed(step, args.steps, max(args.warmup, 3))
     clk = clocks.stop()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"image": st["img"].view(H, W, 3), "loss": st["loss"].reshape(1),
+                                         "samples": torch.tensor([st["samples"]], dtype=torch.int64), **st["grads"]})
     S = st["samples"]
     value = S / ms_step / 1e3
     e2e = None
@@ -542,8 +602,8 @@ def run_ngp(args):
     roofline = {"bound": "hbm", "kernel": dom, "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": traffic_of(dom),
                 "peak_source": peak_src, "algorithmic_bytes_per_launch": per_enc, "avg_launch_ms": t_dom,
                 "kernel_ms": {"grid_encode_fwd": ms_f, "grid_encode_bwd": ms_b},
-                "note": f"one encoder, {S} samples; the {table_mib:.0f} MiB table is L2-resident (126 MB L2), so the gathers / scatters are "
-                        "L2-atomic-bound, not HBM-bound (SURVEY 8d says so); the HBM fraction is reported as asked",
+                "note": f"one encoder, {S} samples; the gathers / scatters are random accesses into a {table_mib:.0f} MiB table "
+                        "(H100 L2: 50 MB), so part of the traffic is served by L2; the HBM fraction is reported as asked",
                 "step_algorithmic_bytes": S * (2 * L * 8 * 2 * 4 + 12 + 4 + 8) * 2}
     cpu = None
     if not args.no_cpu_baseline:
@@ -639,9 +699,11 @@ def run_mesh(args):
     proj = torch.as_tensor(D.gl_perspective(49.1, W / H), dtype=torch.float32)
     mvps = torch.stack([proj @ torch.linalg.inv(torch.as_tensor(GO.orbit_camera(0, 45.0 * k, 1.75), dtype=torch.float32))
                         for k in range(Vn)])            # [8,4,4] clip <- object
+    torch.manual_seed(0)
     gi = torch.rand(Vn, H, W, 3, device=dev)
     tex = torch.rand(1, 1024, 1024, 3, device=dev, requires_grad=True)
     ctx = dr.RasterizeCudaContext()
+    last = {}                 # loss and gradients of the latest step()
 
     def make_step(n_side):
         v_host, f, uv = uv_sphere(n_side, n_side)
@@ -665,7 +727,8 @@ def run_mesh(args):
         pos_dev = (vh.to(dev)[None] @ mvps.to(dev).transpose(1, 2)).contiguous().requires_grad_(True)
 
         def step():
-            chain(pos_dev, plain)
+            loss = chain(pos_dev, plain)
+            last.update(loss=loss.detach(), grad_pos=pos_dev.grad, grad_tex=tex.grad)
             pos_dev.grad = None; tex.grad = None
 
         def e2e_step():      # vertices + view matrices from pinned host memory; loss and vertex gradient back
@@ -692,6 +755,8 @@ def run_mesh(args):
     clocks = Clocks(0)
     ms_step = timed(m["step"], args.steps, max(args.warmup, 3))
     clk = clocks.stop()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"loss": last["loss"].reshape(1), "grad_pos": last["grad_pos"], "grad_tex": last["grad_tex"]})
     value = F * Vn / ms_step / 1e3
     e2e = None
     if not args.no_e2e:

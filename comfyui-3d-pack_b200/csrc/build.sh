@@ -1,9 +1,9 @@
 #!/bin/bash
-# Builds libgs_b200.so in-tree for sm_100a (nvcc cross-compiles without a GPU).
+# Builds libgs_b200.so in-tree for the H100 (sm_90a; nvcc cross-compiles without a GPU).
 set -e
 cd "$(dirname "$0")"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
-ARCH="-gencode arch=compute_100a,code=sm_100a"
+ARCH="-gencode arch=compute_90a,code=sm_90a"
 COMMON="-O3 -std=c++17 -lineinfo -Xcompiler -fPIC $ARCH --expt-relaxed-constexpr ${GS_NVCC_EXTRA}"
 mkdir -p build
 pids=()

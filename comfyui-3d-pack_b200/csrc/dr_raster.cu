@@ -1,7 +1,7 @@
 // Mesh rasterizer: clip-space triangles -> (u, v, z/w, id+1) + barycentric pixel derivatives.
 //
 // Replaces nvdiffrast's dr.rasterize (CudaRaster path; diff_mesh_renderer.py:97, flexicubes_renderer.py:49,
-// mesh_utils.py:531).  B200-first design instead of a port of the bin/coarse/fine software pipeline:
+// mesh_utils.py:531).  GPU-first design instead of a port of the bin/coarse/fine software pipeline:
 //   1. one thread per triangle evaluates 2-D HOMOGENEOUS edge functions (rows of adj([x;y;w])) over its pixel
 //      bounding box — no clipping needed for vertices behind the eye — and resolves visibility with ONE 64-bit
 //      atomicMin per covered pixel on (ordered z/w bits << 32 | triangle id): nearest wins, ties -> lowest id,
@@ -206,7 +206,7 @@ int dr_launch_rasterize_fwd(const float* pos, const int32_t* tri, int B, int V, 
     if (F > 0) {
         const long long nt = (long long)B * F;
         raster_small_kernel<<<(unsigned)((nt + 255) / 256), 256, 0, s>>>((const float4*)pos, tri, B, V, F, H, W, sx, sy, zbuf, queue, qcount);
-        raster_large_kernel<<<148 * 4, 256, 0, s>>>((const float4*)pos, tri, B, V, F, H, W, sx, sy, zbuf, queue, qcount);
+        raster_large_kernel<<<GS_NUM_SMS * 4, 256, 0, s>>>((const float4*)pos, tri, B, V, F, H, W, sx, sy, zbuf, queue, qcount);
         gs_count_launches(2);
     }
     raster_resolve_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, s>>>((const float4*)pos, tri, B, V, H, W, sx, sy, zbuf,

@@ -273,7 +273,7 @@ preprocess_backward_kernel(ViewArgs va, int N, int M, const float* __restrict__ 
         float c[6], R[9], sc[3];
         cov3d_fwd(scales, rotations, cov3D_precomp, va.scale_modifier, idx, c, R, sc);
         ViewB vb{s_view, s_proj, s_cam, va.tanfovx, va.tanfovy, va.focal_x, va.focal_y, va.W, va.H, va.sh_degree};
-        backward_view<false>(vb, M, x, y, z, c, sg[idx].g, sg[idx].c, sg[idx].k, my_sh, my_sh, shs != nullptr, A);
+        backward_view<false>(vb, M, x, y, z, c, sg_f4(sg[idx].g), sg_f4(sg[idx].c), sg_f4(sg[idx].k), my_sh, my_sh, shs != nullptr, A);
         if (cov3D_precomp == nullptr) cov3d_bwd(A.dcv, R, sc, va.scale_modifier, rotations + 4 * (size_t)idx, dsc, dq);
     } else if (live && shs != nullptr) {
         for (int k = 0; k < row; k++) my_sh[k] = 0.f;
@@ -328,12 +328,12 @@ preprocess_backward_multi_kernel(const float* __restrict__ views, int V, int W, 
         for (int v = 0; v < V; v++) vis |= (radii[(size_t)v * N + idx] > 0 ? 1u : 0u) << v;
         any_vis = vis != 0;
         float4 ng = make_float4(0.f, 0.f, 0.f, 0.f), nc = ng, nk = ng;
-        if (vis) { const SplatGrad* q = sg + (size_t)(__ffs(vis) - 1) * N + idx; ng = q->g; nc = q->c; nk = q->k; }
+        if (vis) { const SplatGrad* q = sg + (size_t)(__ffs(vis) - 1) * N + idx; ng = sg_f4(q->g); nc = sg_f4(q->c); nk = sg_f4(q->k); }
         while (vis) {
             const int v = __ffs(vis) - 1;
             vis &= vis - 1;
             const float4 cg = ng, cc = nc, ck = nk;
-            if (vis) { const SplatGrad* q = sg + (size_t)(__ffs(vis) - 1) * N + idx; ng = q->g; nc = q->c; nk = q->k; }
+            if (vis) { const SplatGrad* q = sg + (size_t)(__ffs(vis) - 1) * N + idx; ng = sg_f4(q->g); nc = sg_f4(q->c); nk = sg_f4(q->k); }
             const float* vw = s_views + v * 40;
             const float tfx = vw[38], tfy = vw[39];
             ViewB vb{vw, vw + 16, vw + 32, tfx, tfy, (float)W / (2.0f * tfx), (float)H / (2.0f * tfy), W, H, sh_degree};

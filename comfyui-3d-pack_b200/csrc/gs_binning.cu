@@ -2,7 +2,7 @@
 // debug reconstruction of the package's 64-bit keys.
 //
 // Replaces duplicateWithKeys / identifyTileRanges of diff_gaussian_rasterization
-// (SURVEY.md App. A.1.5).  B200-first restructuring: the package sorts K*N
+// (SURVEY.md App. A.1.5).  GPU-first restructuring: the package sorts K*N
 // 64-bit (tile|depth) keys in one go; here the N Gaussians are depth-sorted
 // FIRST (N 32-bit keys), pairs are emitted in that order, and only the tile id
 // (ceil(log2(tiles)) bits) is sorted over the K*N pairs.  Both sorts are stable,

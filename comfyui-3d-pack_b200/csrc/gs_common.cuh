@@ -1,8 +1,11 @@
-// Shared definitions for the sm_100a Gaussian-splatting kernels.
+// Shared definitions for the sm_90a (H100) Gaussian-splatting kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+
+// SMs of an H100 SXM: capped and persistent grids are sized as small multiples of it.
+#define GS_NUM_SMS 132
 
 #define GS_TILE 16
 #define GS_TILE_PIX 256
@@ -31,13 +34,21 @@ struct __align__(16) SplatRec {
     float4 k;   // r, g, b, tiles_touched(uint bits)
 };
 
-// Per-Gaussian gradient accumulator filled by the composite backward (atomics).
+// Per-Gaussian gradient accumulator filled by the composite backward (atomics).  Every tile adds its fp32 partial sums
+// in whatever order the CTAs finish.  In fp32 that order changes cancelling sums (the rotation gradient of an isotropic
+// splat is all cancellation) by up to an ulp of the largest partial, i.e. by more than the sum itself; the fp64 sums
+// here keep the order-dependent error ~2^-29 below that, so the fp32 values read back (sg_f4) differ between runs only
+// where a sum lands that close to an fp32 rounding boundary -- not a guarantee, in practice bit-identical.
 struct __align__(16) SplatGrad {
     // raw moment sums over the pixels a splat was blended into, w = dL/dG * G, d = mean2D - pixel:
-    float4 g;   // sum w*dx, sum w*dy, dL/ddepth, -
-    float4 c;   // sum w*dx*dx, sum w*dx*dy, sum w*dy*dy, dL/dopacity
-    float4 k;   // dL/dr, dL/dg, dL/db, -
+    double4 g;   // sum w*dx, sum w*dy, dL/ddepth, -
+    double4 c;   // sum w*dx*dx, sum w*dx*dy, sum w*dy*dy, dL/dopacity
+    double4 k;   // dL/dr, dL/dg, dL/db, -
 };
+
+__device__ __forceinline__ float4 sg_f4(const double4 d) {
+    return make_float4((float)d.x, (float)d.y, (float)d.z, (float)d.w);
+}
 
 struct ViewConst {
     float view[16];

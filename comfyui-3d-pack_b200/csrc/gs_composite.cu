@@ -8,20 +8,18 @@
 // Called where main_3DGS_renderer.py:927-936 calls the rasterizer and where
 // loss.backward() (main_3DGS.py:205) reaches its backward.
 //
-// Both kernels are instruction-issue bound (the 48 B splat records live in L2),
-// so the design minimises issued instructions per (pixel, splat) and takes the
-// record staging off the math warps:
-//  * one CTA per 16x16 tile = 4 math warps + 1 producer warp.  Math warp w owns
+// Both kernels are meant to be instruction-issue bound (48 B splat records, gathered through L2),
+// so the design minimises issued instructions per (pixel, splat):
+//  * one CTA per 16x16 tile = 4 warps.  Warp w owns
 //    the 8x8 quadrant (w&1, w>>1); every lane owns TWO pixels (x, y) and (x, y+4),
-//    so dx is shared and all per-pixel arithmetic is issued as packed f32x2
-//    (fma.rn.f32x2 / mul / add -> FFMA2 / FMUL2 / FADD2, scalar operands
-//    broadcast by the instruction itself);
-//  * the producer warp gathers the tile's records with one cp.async.bulk (TMA,
-//    UBLKCP) of 48 B per record into a ring of shared-memory stages; completion
-//    is tracked by an mbarrier per stage (expect_tx / complete_tx), math warps
-//    release a stage with one mbarrier.arrive per warp.  There is no
-//    __syncthreads() in the main loops;
-//  * each math warp decides by itself which records of a stage can reach
+//    so dx and every per-splat operand are loaded and set up once for two
+//    pixels (the pixel pair is carried as one 64-bit register pair);
+//  * the tile's records are gathered by three 16 B cp.async per record (or, with
+//    GS_B200_GATHER=tma, one 48 B cp.async.bulk) into a ring of shared-memory
+//    stages, each completed on an mbarrier; a warp releases a stage with one
+//    shared-memory atomic and the last of the four to release it refills it.
+//    There is no __syncthreads() in the main loops;
+//  * each warp decides by itself which records of a stage can reach
 //    alpha >= 1/255 inside its quadrant (exact minimum of the quadratic form over
 //    the 8x8 rectangle + slack): one test per lane and record, four ballots per
 //    128-record stage, then the warp walks only the set bits;
@@ -32,7 +30,8 @@
 //    pixel-local coordinates, four colour/depth sums against per-pixel upstream
 //    gradients) with plain FFMAs and no cross-lane traffic beyond one final
 //    shfl.xor — the 12-SHFL transpose reduction per (warp, splat) of round 1 is
-//    gone.  One red.global.add per value and (quadrant, splat) leaves the CTA.
+//    gone.  One fp64 red.global.add per value and (quadrant, splat) leaves the CTA
+//    (SplatGrad in gs_common.cuh says why fp64).
 #include "gs_common.cuh"
 #include <stdlib.h>
 
@@ -47,18 +46,20 @@ constexpr uint32_t REC_BYTES = 48;
 constexpr uint32_t STAGE_BYTES = BATCH * REC_BYTES;
 constexpr float ALPHA_MIN = 1.0f / 255.0f;
 
-// ---- packed f32x2 helpers (sm_100a: FFMA2 / FMUL2 / FADD2) ------------------------------------
+// ---- pixel-pair helpers ---------------------------------------------------------------------------
+// The two pixels of a lane travel as one 64-bit register pair.  sm_90 has no packed f32x2 arithmetic, so each
+// helper issues two scalar IEEE operations; the explicit _rn intrinsics keep the rounding of every step (no FMA
+// contraction of a mul followed by an add), so both pixels get exactly the results a packed instruction would give.
 __device__ __forceinline__ u64 pk(float lo, float hi) { u64 r; asm("mov.b64 %0, {%1,%2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
 __device__ __forceinline__ u64 bc(float a) { return pk(a, a); }
 __device__ __forceinline__ float lo(u64 v) { float a, b; asm("mov.b64 {%0,%1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); return a; }
 __device__ __forceinline__ float hi(u64 v) { float a, b; asm("mov.b64 {%0,%1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); return b; }
-__device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) { u64 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
-// acc = a * b + acc with the accumulator as a read-write operand (keeps loop-carried sums in one register pair)
-__device__ __forceinline__ void fma2_acc(u64& acc, u64 a, u64 b) { asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc) : "l"(a), "l"(b)); }
-__device__ __forceinline__ void add2_acc(u64& acc, u64 a) { asm("add.rn.f32x2 %0, %0, %1;" : "+l"(acc) : "l"(a)); }
-__device__ __forceinline__ u64 mul2(u64 a, u64 b) { u64 r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ u64 add2(u64 a, u64 b) { u64 r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ u64 sub2(u64 a, u64 b) { u64 r; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
+__device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) {
+    return pk(__fmaf_rn(lo(a), lo(b), lo(c)), __fmaf_rn(hi(a), hi(b), hi(c)));
+}
+__device__ __forceinline__ u64 mul2(u64 a, u64 b) { return pk(__fmul_rn(lo(a), lo(b)), __fmul_rn(hi(a), hi(b))); }
+__device__ __forceinline__ u64 add2(u64 a, u64 b) { return pk(__fadd_rn(lo(a), lo(b)), __fadd_rn(hi(a), hi(b))); }
+__device__ __forceinline__ u64 sub2(u64 a, u64 b) { return pk(__fsub_rn(lo(a), lo(b)), __fsub_rn(hi(a), hi(b))); }
 
 __device__ __forceinline__ float4 lds128(uint32_t addr) {
     float4 v;
@@ -105,8 +106,10 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
-__device__ __forceinline__ void red_add_v4(float* addr, float4 v) {      // 16-byte aligned global address
-    asm volatile("red.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
+// adds the first n components of v to an fp64 double4 of a SplatGrad record (sm_90 has no vector fp64 red)
+__device__ __forceinline__ void red_add_d4(double* addr, float4 v, int n) {
+    atomicAdd(addr, (double)v.x); atomicAdd(addr + 1, (double)v.y); atomicAdd(addr + 2, (double)v.z);
+    if (n == 4) atomicAdd(addr + 3, (double)v.w);
 }
 __device__ __forceinline__ uint32_t ld_volatile_s32(uint32_t addr) {
     uint32_t v;
@@ -190,9 +193,9 @@ struct RingState {
 // gather of one stage: ids (coalesced LDG), then per record either three 16 B cp.async (LDGSTS) per lane with one
 // cp.async.mbarrier.arrive.noinc per lane (the stage's mbarrier expects 32 arrivals) -- the default -- or
 // (GS_B200_GATHER=tma) ONE 48 B bulk copy through the TMA engine (UBLKCP; completion = bytes counted on the stage's
-// mbarrier, which one expect_tx arrival arms).  Both were measured on B200 (DESIGN 5.1): UBLKCP takes its operands from
-// uniform registers, so a per-lane gather serialises into a ~9-instruction loop per record inside the issuing warp,
-// whereas the three LDGSTS are one warp-wide instruction each -- the whole step is 7.6 % faster with LDGSTS.
+// mbarrier, which one expect_tx arrival arms).  UBLKCP takes its operands from uniform registers, so a per-lane
+// gather serialises into a ~9-instruction loop per record inside the issuing warp, whereas the three LDGSTS are one
+// warp-wide instruction each.
 template <bool KEEP_IDS, bool TMA>
 __device__ __forceinline__ void produce_stage(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ list, int n,
                                               uint32_t s_rec, uint32_t s_ids, uint32_t bar, int lane) {
@@ -509,11 +512,11 @@ __device__ __noinline__ void flush_queue(uint32_t q_base, uint32_t coef_base, ui
 #undef XADD
     }
     if (slot < nq) {
-        float* dst = reinterpret_cast<float*>(sg + gid);
+        double* dst = reinterpret_cast<double*>(sg + gid);
         // pixel = centre + L, d = mean2D - pixel = u - L with u = mean2D - centre
         const float u = si.x - Xc, v = si.y - Yc, o = si.w;
-        // the ten sums of the splat = the three float4 of its SplatGrad record; one red.global.add.v4.f32 per float4
-        // (3 vector reds per (quadrant, splat) instead of 10 scalar ones), shared between the parts of the slot
+        // the ten sums of the splat = the three double4 of its SplatGrad record (ten fp64 reds per (quadrant, splat)),
+        // shared between the parts of the slot
         const float4 qg = make_float4(o * (u * M0 - M1),                                   // sum w dx
                                       o * (v * M0 - My),                                   // sum w dy
                                       Cd, 0.f);                                            // dL/ddepth
@@ -523,10 +526,10 @@ __device__ __noinline__ void flush_queue(uint32_t q_base, uint32_t coef_base, ui
                                       M0);                                                 // dL/dopacity (sum G dL/dalpha)
         const float4 qk = make_float4(Cr, Cg, Cb, 0.f);                                    // dL/drgb
         if (Q::PARTS == 2) {
-            red_add_v4(dst + (part == 0 ? 0 : 8), part == 0 ? qg : qk);
-            if (part == 0) red_add_v4(dst + 4, qc);
+            red_add_d4(dst + (part == 0 ? 0 : 8), part == 0 ? qg : qk, 3);
+            if (part == 0) red_add_d4(dst + 4, qc, 4);
         } else {
-            if (part < 3) red_add_v4(dst + 4 * part, part == 0 ? qg : (part == 1 ? qc : qk));
+            if (part < 3) red_add_d4(dst + 4 * part, part == 0 ? qg : (part == 1 ? qc : qk), part == 1 ? 4 : 3);
         }
     }
 }
@@ -732,7 +735,7 @@ constexpr size_t bwd_smem_bytes(int stages, int slots) {
            8 * (size_t)stages + 4 * (size_t)stages + 16;
 }
 
-bool gather_tma() {       // GS_B200_GATHER=tma selects the TMA bulk-copy gather (measured slower than the cp.async default)
+bool gather_tma() {       // GS_B200_GATHER=tma selects the TMA bulk-copy gather instead of the cp.async default
     static const bool tma = []() { const char* e = getenv("GS_B200_GATHER"); return e && e[0] == 't'; }();
     return tma;
 }
@@ -789,9 +792,7 @@ int gs_launch_render_backward(const ViewArgs& va, const SplatRec* recs, const ui
                               SplatGrad* sg, cudaStream_t s) {
     if (use_r1()) return gs_launch_render_backward_r1(va, recs, point_list, ranges, n_contrib, final_T, dL_dcolor, dL_ddepth, dL_dalpha, sg, s);
     dim3 grid(va.tiles_x, va.tiles_y);
-    // Measured on B200 (DESIGN 5.1) and no longer instantiated: 8-slot queues with 5-6 CTAs/SM (flush overhead), forced
-    // 5 CTAs/SM at 16 slots (spills), a per-visit warp vote around the sequential half (the branch costs more than the 5 %
-    // dead visits).  Left selectable: ring depth (GS_B200_BWD_STAGES 2/3) and the TMA gather (GS_B200_GATHER=tma).
+    // Selectable: ring depth (GS_B200_BWD_STAGES 2/3) and the TMA gather (GS_B200_GATHER=tma).
     static const int stages = env_int("GS_B200_BWD_STAGES", 2);
     static const bool pair = env_int("GS_B200_BWD_PAIR", 1) != 0;      // both visits of an iteration unconditional (second masked)
 #define BWD(ST, TM, PR)                                                                                                    \

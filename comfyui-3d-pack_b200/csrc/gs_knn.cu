@@ -207,7 +207,7 @@ int gs_launch_knn(const float* points, int N, float* out, cudaStream_t s) {
     void* sort_scratch = (void*)(((uintptr_t)(cell_start + ncells + 1) + 255) & ~(uintptr_t)255);
     const int init[7] = {0x7fffffff, 0x7fffffff, 0x7fffffff, (int)0x80000000, (int)0x80000000, (int)0x80000000, 0};
     GS_CUDA_CHECK(cudaMemcpyAsync(box, init, sizeof(init), cudaMemcpyHostToDevice, s));
-    knn_bbox_kernel<<<std::min((N + 255) / 256, 148 * 8), 256, 0, s>>>(points, N, box);
+    knn_bbox_kernel<<<std::min((N + 255) / 256, GS_NUM_SMS * 8), 256, 0, s>>>(points, N, box);
     int hbox[7];
     GS_CUDA_CHECK(cudaMemcpyAsync(hbox, box, sizeof(hbox), cudaMemcpyDeviceToHost, s));
     GS_CUDA_CHECK(cudaStreamSynchronize(s));

@@ -6,8 +6,8 @@
 // power>0 or alpha<1/255; stop WITHOUT blending when T(1-alpha) < 1e-4;
 // color = C + T*bg, depth = sum(depth*alpha*T), alpha_out = sum(alpha*T).
 //
-// Design (sm_100a) — both kernels are instruction-issue bound, not HBM bound
-// (the splat records, 48 MB, live in the 126 MB L2), so everything here is about
+// Design — both kernels are meant to be instruction-issue bound, not HBM bound
+// (48 B splat records, gathered through L2), so everything here is about
 // issuing fewer instructions per (pixel, splat):
 //  * one CTA per 16x16 tile, 8 warps, each warp owns an 8x4 pixel sub-rect;
 //  * a batch of 256 records (3 x LDG.128 each) is staged in shared memory as
@@ -25,7 +25,7 @@
 //    the per-Gaussian preprocess backward; the 10 sums are reduced over the 32
 //    lanes with a TRANSPOSE butterfly (12 SHFL instead of 50) that leaves each
 //    total in its own lane, so ONE red.global.add instruction with 10 active
-//    lanes updates the 48 B gradient record.
+//    lanes updates the fp64 gradient record.
 #include "gs_common.cuh"
 #include <stdlib.h>
 
@@ -218,7 +218,7 @@ render_backward_kernel(ViewArgs va, const SplatRec* __restrict__ recs, const uin
     const int sub = (h8 ? 3 : 0) + (h4 ? 2 : 0) + (h2 ? 1 : 0);
     const bool my_valid = !(lane & 1) && !(h8 && h4) && !(!h8 && h4 && h2);
     const int vi = (h16 ? 5 : 0) + sub;                       // 0..9
-    const int my_off = vi + (vi >= 3);                        // float offset inside SplatGrad (skips g.w)
+    const int my_off = vi + (vi >= 3);                        // element offset inside SplatGrad (skips g.w)
 
     if (tid == 0) s_max = 0;
     __syncthreads();
@@ -294,7 +294,7 @@ render_backward_kernel(ViewArgs va, const SplatRec* __restrict__ recs, const uin
                 const float s0 = xstage(t0, t2, h4, 4), s1 = xstage(t1, 0.f, h4, 4);
                 float r = xstage(s0, s1, h2, 2);
                 r += __shfl_xor_sync(0xFFFFFFFFu, r, 1);
-                if (my_valid) atomicAdd(reinterpret_cast<float*>(sg + s_id[j]) + my_off, r);
+                if (my_valid) atomicAdd(reinterpret_cast<double*>(sg + s_id[j]) + my_off, (double)r);
             }
         }
     }

@@ -147,8 +147,8 @@ rs_onesweep(const uint32_t* __restrict__ keys_in, uint32_t* __restrict__ keys_ou
 #pragma unroll
     for (int i = 0; i < RS_ITEMS; i++) {
         const uint32_t d = (k[i] >> shift) & 0xFF;
-        // lanes holding the same digit.  NOT match.any: MATCH is executed by a shared unit at ~128 cycles per
-        // warp instruction on sm_100 (measured: it alone accounted for the whole pass time); 8 VOTE + 8 LOP3 are free.
+        // lanes holding the same digit.  NOT match.any: MATCH is a slow, shared-unit warp instruction, while
+        // 8 VOTE + 8 LOP3 issue at full rate.
         uint32_t peers = 0xFFFFFFFFu;
 #pragma unroll
         for (int b = 0; b < 8; b++) {
@@ -378,7 +378,7 @@ int gs_sort_pairs_u32_biased(uint32_t* keys, uint32_t* keys_alt, uint32_t* vals,
     uint32_t* trivial = tickets + 8;
     uint32_t* status = tickets + 64;
     GS_CUDA_CHECK(cudaMemsetAsync(scratch, 0, gs_sort_scratch_bytes(n) - (size_t)(RS_MAX_PASSES - npasses) * parts * RS_RADIX * 4, s));
-    int64_t hb = (n + RS_THREADS * 8 - 1) / (RS_THREADS * 8); int hblocks = (int)(hb < 148 * 8 ? hb : 148 * 8);
+    int64_t hb = (n + RS_THREADS * 8 - 1) / (RS_THREADS * 8); int hblocks = (int)(hb < GS_NUM_SMS * 8 ? hb : GS_NUM_SMS * 8);
     rs_histogram<<<hblocks, RS_THREADS, 0, s>>>(keys, n, ghist, begin_bit, npasses, key_bias);
     rs_scan_hist<<<npasses, RS_RADIX, 0, s>>>(ghist, trivial, (uint32_t)n);
     uint32_t *kin = keys, *kout = keys_alt, *vin = vals, *vout = vals_alt;

@@ -185,7 +185,7 @@ int launch_bwd(const float* X, long long N, const float* W1, const float* W2, co
     const size_t smem = (size_t)(2 * DIN * H + 4 * H + MT * (DIN + 1) + 2 * MT * (H + 1) + MT * 4) * 4;
     static bool set = false;
     if (!set) { cudaFuncSetAttribute(mlp2_bwd_kernel<DIN, H, DOUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); set = true; }
-    const long long tiles_ = (N + MT - 1) / MT; const int grid = (int)(tiles_ < 148 * 3 ? tiles_ : 148 * 3);
+    const long long tiles_ = (N + MT - 1) / MT; const int grid = (int)(tiles_ < GS_NUM_SMS * 3 ? tiles_ : GS_NUM_SMS * 3);
     mlp2_bwd_kernel<DIN, H, DOUT><<<grid, MT, smem, s>>>(X, N, W1, W2, GY, GX, GW1, GW2);
     return 0;
 }

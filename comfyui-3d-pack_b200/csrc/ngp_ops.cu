@@ -2,8 +2,8 @@
 // ray marching, packed volume-rendering weights and per-ray accumulation.
 //
 // Replace kiui.gridencoder (torch-ngp) and nerfacc for Instant_NGP.py:101-156,195 (SURVEY.md App. A.3-A.4).
-// Bounds: the two hash tables (<= 2 x 12 levels x 4 MiB) are L2-resident on B200 (126 MB L2), so encode /
-// scatter are L2-gather bound, not HBM bound; marching is ALU-bound on a 32 KB bit grid held in shared memory;
+// Bounds: encode / scatter are random gathers / reds into the two hash tables (<= 2 x 12 levels x 4 MiB, close
+// to the 50 MB L2 of an H100); marching is ALU-bound on a 32 KB bit grid held in shared memory;
 // weights / accumulate stream the packed samples once.
 // fp32 operation order of everything that decides an INTEGER output (corner indices, the packed sample list)
 // is pinned with __fmul_rn/__fadd_rn/__fdiv_rn to match oracle/ngp_oracle.py bit for bit.

@@ -31,7 +31,7 @@ ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_int32, C.c_size_t)
 
 if not os.path.exists(LIB_PATH):
     raise ImportError(
-        f"{LIB_PATH} is missing: the sm_100a CUDA library has not been built. "
+        f"{LIB_PATH} is missing: the sm_90a CUDA library has not been built. "
         "Run `python __graft_entry__.py` (or comfyui-3d-pack_b200/csrc/build.sh). There is no CPU fallback.")
 
 lib = C.CDLL(LIB_PATH)

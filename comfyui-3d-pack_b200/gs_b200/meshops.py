@@ -3,7 +3,7 @@
     RasterizeCudaContext / RasterizeGLContext, rasterize, interpolate, texture, antialias
 
 Call sites: MVs_Algorithms/DiffRastMesh/diff_mesh_renderer.py:45-138, FlexiCubes/flexicubes_renderer.py:46-66,
-FlexiCubes/util.py:90-93, mesh_processer/mesh_utils.py:522-541.  All compute is the sm_100a library behind
+FlexiCubes/util.py:90-93, mesh_processer/mesh_utils.py:522-541.  All compute is the sm_90a library behind
 include/dr_b200.h; PyTorch is device memory + autograd glue.  No CPU path.
 """
 import ctypes as C

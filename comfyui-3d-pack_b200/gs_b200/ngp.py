@@ -1,6 +1,6 @@
 """Host-side mirror of the kiui.gridencoder / kiui.nn / nerfacc surface used by the reference's Instant-NGP node
 (MVs_Algorithms/NeRF/Instant_NGP.py:20-35,101-156,195; LGM/nerf_marching_cubes_converter.py:56-59,98-154).
-Compute is the sm_100a library behind include/ngp_b200.h; PyTorch is memory, autograd glue, and the tiny
+Compute is the sm_90a library behind include/ngp_b200.h; PyTorch is memory, autograd glue, and the tiny
 MLPs (plain library GEMMs).  No CPU path."""
 import ctypes as C
 import math

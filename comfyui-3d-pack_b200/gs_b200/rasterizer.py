@@ -12,7 +12,7 @@ TriplaneGaussian/models/renderer.py:209-304, TRELLIS gaussian_render.py:62-137):
         -> (color[3,H,W], radii[N] int32, depth[1,H,W], alpha[1,H,W])
 
 PyTorch is plumbing only (device memory, streams, autograd glue); all compute is
-the sm_100a library behind include/gs_b200.h.  No CPU path exists.
+the sm_90a library behind include/gs_b200.h.  No CPU path exists.
 """
 from typing import NamedTuple, Optional
 import ctypes as C

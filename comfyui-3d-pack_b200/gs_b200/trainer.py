@@ -1,4 +1,4 @@
-"""B200-native optimisation loop around the rasterizer: the fast path for what GaussianModel +
+"""H100-native optimisation loop around the rasterizer: the fast path for what GaussianModel +
 GaussianSplatting3D.training do in the reference (MVs_Algorithms/GaussianSplatting/main_3DGS_renderer.py:236-781,
 main_3DGS.py:86-232).  The reference's own Python runs unmodified over the `diff_gaussian_rasterization` shim; this
 module is the packed-layout alternative: one raw-parameter buffer, fused activation, multi-view pipelined

@@ -1,5 +1,5 @@
 /*
- * dr_b200.h — C ABI of the B200-native mesh rasterisation ops (the nvdiffrast surface ComfyUI-3D-Pack uses).
+ * dr_b200.h — C ABI of the H100-native mesh rasterisation ops (the nvdiffrast surface ComfyUI-3D-Pack uses).
  *
  * Replaces, for the reference's call sites, the torch ops of the un-vendored package `nvdiffrast.torch`
  * (0.3.3, my-reqs.txt:74):

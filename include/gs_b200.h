@@ -1,5 +1,5 @@
 /*
- * gs_b200.h — C ABI of the B200-native 3D Gaussian-splatting rasterizer.
+ * gs_b200.h — C ABI of the H100-native 3D Gaussian-splatting rasterizer.
  *
  * Drop-in boundary for the path ComfyUI-3D-Pack reaches through the third-party
  * Python package `diff_gaussian_rasterization` (ashawkey fork), whose two
@@ -93,7 +93,7 @@ int32_t gs_b200_set_tile_culling(int32_t mode);
 int32_t gs_b200_get_tile_culling(void);
 
 /* Measurement switch (no reference counterpart): which tile-composite kernels run.  0 (default): the round-2
- * kernels (gs_composite.cu: two pixels per lane in packed f32x2, cp.async-fed mbarrier ring, queued gradient phase);
+ * kernels (gs_composite.cu: two pixels per lane, cp.async-fed mbarrier ring, queued gradient phase, fp64 gradient sums);
  * 1: the round-1 kernels (gs_render.cu), kept for A/B timing.  Results agree (images bit for bit).
  * Initial value from the environment variable GS_B200_COMPOSITE ("r1" selects 1). */
 int32_t gs_b200_debug_set_composite(int32_t mode);

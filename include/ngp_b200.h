@@ -1,5 +1,5 @@
 /*
- * ngp_b200.h — C ABI of the B200-native Instant-NGP path: multiresolution hash-grid encoding, occupancy-grid
+ * ngp_b200.h — C ABI of the H100-native Instant-NGP path: multiresolution hash-grid encoding, occupancy-grid
  * ray marching, packed volume-rendering weights and per-ray accumulation.
  *
  * Replaces, for MVs_Algorithms/NeRF/Instant_NGP.py (and Gen_3D_Modules/LGM/nerf_marching_cubes_converter.py),

@@ -1,7 +1,7 @@
 """CPU oracle for the mesh path (nvdiffrast surface) — TEST INFRASTRUCTURE ONLY.
 
     PARITY UNPINNED: nvdiffrast 0.3.3 (my-reqs.txt:74, dependencies.txt:3) is an un-vendored third-party
-    package, absent from /root/reference and from this image; the reference ships no tests or golden
+    package, absent from the reference source tree and not installable offline; the reference ships no tests or golden
     images for it (SURVEY.md §4, §8c).
 
 Restates the published algorithms (Laine et al. 2020, "Modular Primitives for High-Performance

@@ -2,8 +2,8 @@
 — TEST INFRASTRUCTURE ONLY.
 
     PARITY UNPINNED: kiui 0.2.14 (`kiui.gridencoder`, torch-ngp's grid encoder; my-reqs.txt:50) and nerfacc
-    0.5.3 (my-reqs.txt:69) are un-vendored third-party packages, absent from /root/reference and from this
-    image; the reference has no tests or golden vectors for them (SURVEY.md §4, §8c).
+    0.5.3 (my-reqs.txt:69) are un-vendored third-party packages, absent from the reference source tree and not
+    installable offline; the reference has no tests or golden vectors for them (SURVEY.md §4, §8c).
 
 Restates the published algorithms (Müller et al. 2022 multiresolution hash encoding as implemented by
 torch-ngp; Li et al. 2023 nerfacc occupancy-grid sampling and packed volume rendering; SURVEY.md App. A.3-A.4)

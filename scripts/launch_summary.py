@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Summarise an `ncu --metrics gpu__time_duration.sum --csv --log-file X.csv <cmd>` launch list: per kernel name the
 launch count, average duration and share of the total kernel time (cold-cache, serialised: compare SHARES).
-usage: python scripts/launch_summary.py gpurun_out/launches.csv "header line" > profiles/rN_launch_list_summary.txt"""
+usage: python scripts/launch_summary.py launches.csv "header line" > launch_list_summary.txt"""
 import csv
 import sys
 from collections import defaultdict

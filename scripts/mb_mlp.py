@@ -1,5 +1,5 @@
-import sys
-sys.path.insert(0, '/root/repo'); sys.path.insert(0, '/root/repo/comfyui-3d-pack_b200')
+import os, sys
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'comfyui-3d-pack_b200'))
 import torch
 from kiui.nn import MLP
 dev = torch.device('cuda:0')

@@ -1,5 +1,5 @@
 import os, sys
-sys.path.insert(0, '/root/repo'); sys.path.insert(0, '/root/repo/comfyui-3d-pack_b200')
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'comfyui-3d-pack_b200'))
 import torch
 from kiui.gridencoder import GridEncoder
 dev = torch.device('cuda:0')

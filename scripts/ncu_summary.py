@@ -1,5 +1,5 @@
 """Summarise an .ncu-rep (read here, no GPU): key raw metrics per kernel launch + top stall reasons.
-usage: python scripts/ncu_summary.py gpurun_out/prof.ncu-rep [out.txt]"""
+usage: python scripts/ncu_summary.py prof.ncu-rep [out.txt]"""
 import csv, io, subprocess, sys
 rep = sys.argv[1]
 raw = subprocess.run(["ncu", "-i", rep, "--page", "raw", "--csv"], capture_output=True, text=True).stdout

@@ -1,5 +1,5 @@
 #!/bin/bash
-# compute-sanitizer passes over small GPU cases (memcheck + racecheck); run under gpurun.
+# compute-sanitizer passes over small GPU cases (memcheck + racecheck); run on a GPU machine.
 set -o pipefail
 cd "$(dirname "$0")/.."
 T='tests/test_gpu_parity.py::test_onesweep_sort_matches_stable_sort tests/test_gpu_parity.py::test_empty_culled_and_offscreen_inputs tests/test_gpu_parity.py::test_colors_precomp_and_cov3d_precomp_paths tests/test_gpu_mesh.py::test_topology_matches_oracle tests/test_gpu_mesh.py::test_texture_wrap_clamp_and_gradients tests/test_gpu_ngp.py::test_weights_accumulate_forward_backward'

@@ -1,6 +1,6 @@
 #!/bin/bash
 # compute-sanitizer over the kernels added late in round 1 (tile culling, in-pipeline loss, grid kNN, run-reduced
-# hash-grid scatter, flat Adam); run under gpurun.
+# hash-grid scatter, flat Adam); run on a GPU machine.
 set -o pipefail
 cd "$(dirname "$0")/.."
 cat > /tmp/new_case.py <<'PY'

@@ -1,6 +1,6 @@
-"""Generates tests/golden/*.npz.  Run HERE (build container), where /root/reference exists:
+"""Generates tests/golden/*.npz from a checkout of ComfyUI-3D-Pack named by $COMFYUI_3D_PACK:
 
-    python tests/golden/make_golden.py
+    COMFYUI_3D_PACK=/path/to/ComfyUI-3D-Pack python tests/golden/make_golden.py
 
 Two kinds of fixtures:
  (1) ref_*.npz  — outputs of the REFERENCE's own pure-PyTorch helpers that sit on the rasterizer path
@@ -18,7 +18,7 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REF = "/root/reference"
+REF = os.environ["COMFYUI_3D_PACK"]
 sys.path.insert(0, ROOT)
 
 

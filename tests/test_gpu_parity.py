@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: pytest -m gpu).  Every test goes through the C ABI
+"""GPU parity tests (run on an H100: pytest -m gpu).  Every test goes through the C ABI
 (libgs_b200.so via ctypes); the CPU oracle is the checker.
 
 Tolerances (BASELINE.json north_star): rendered RGBA within 1e-4 abs, gradients within 1e-3 relative,
