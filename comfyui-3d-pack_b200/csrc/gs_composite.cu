@@ -14,8 +14,8 @@
 //    the 8x8 quadrant (w&1, w>>1); every lane owns TWO pixels (x, y) and (x, y+4),
 //    so dx and every per-splat operand are loaded and set up once for two
 //    pixels (the pixel pair is carried as one 64-bit register pair);
-//  * the tile's records are gathered by three 16 B cp.async per record (or, with
-//    GS_B200_GATHER=tma, one 48 B cp.async.bulk) into a ring of shared-memory
+//  * the tile's records are gathered by three 16 B cp.async per record (or, in the
+//    forward with GS_B200_GATHER=tma, one 48 B cp.async.bulk) into a ring of shared-memory
 //    stages, each completed on an mbarrier; a warp releases a stage with one
 //    shared-memory atomic and the last of the four to release it refills it.
 //    There is no __syncthreads() in the main loops;
@@ -25,13 +25,15 @@
 //    128-record stage, then the warp walks only the set bits;
 //  * backward, per visit, only TWO values per pixel leave the lanes:
 //    G*dL/dalpha and alpha*T.  They are queued in shared memory ([pixel][slot])
-//    and, every 16 visits, a second phase with lanes = (slot, half-quadrant)
+//    and, every 16 visits and at the end of each stage, a second phase with lanes = (slot, half-quadrant)
 //    turns them into the ten per-splat sums (six image moments of G*dL/dalpha in
 //    pixel-local coordinates, four colour/depth sums against per-pixel upstream
 //    gradients) with plain FFMAs and no cross-lane traffic beyond one final
 //    shfl.xor — the 12-SHFL transpose reduction per (warp, splat) of round 1 is
-//    gone.  One fp64 red.global.add per value and (quadrant, splat) leaves the CTA
-//    (SplatGrad in gs_common.cuh says why fp64).
+//    gone.  The sums stop in a per-stage block of fp32 partials in shared memory; when
+//    the stage is released, its last warp adds the partials of the (up to four) quadrants
+//    of each splat in fp64, in fixed warp order, and ONE fp64 red.global.add per value and
+//    (tile, splat) leaves the CTA (SplatGrad in gs_common.cuh says why fp64).
 #include "gs_common.cuh"
 #include <stdlib.h>
 
@@ -106,10 +108,18 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
-// adds the first n components of v to an fp64 double4 of a SplatGrad record (sm_90 has no vector fp64 red)
-__device__ __forceinline__ void red_add_d4(double* addr, float4 v, int n) {
-    atomicAdd(addr, (double)v.x); atomicAdd(addr + 1, (double)v.y); atomicAdd(addr + 2, (double)v.z);
-    if (n == 4) atomicAdd(addr + 3, (double)v.w);
+__device__ __forceinline__ float lds32(uint32_t addr) {
+    float v;
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
+    return v;
+}
+__device__ __forceinline__ uint32_t ldsu32(uint32_t addr) {
+    uint32_t v;
+    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
+    return v;
+}
+__device__ __forceinline__ void sts32(uint32_t addr, float a) {
+    asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(a) : "memory");
 }
 __device__ __forceinline__ uint32_t ld_volatile_s32(uint32_t addr) {
     uint32_t v;
@@ -458,26 +468,31 @@ template <int SLOTS> struct QGeom {
     static constexpr int PARTS = 32 / SLOTS;       // lanes = (slot, part); a part owns SLOTS consecutive lane rows
 };
 
+// Partial block of one ring stage: the ten per-splat sums of every (warp, record) the warp visited, fp32,
+// [warp][value][record] (value-major, so the combine's lanes = records read consecutive words), followed by the warps'
+// hit masks of the stage [warp][BATCH / 32], which say which partials exist (the block is never cleared).
+constexpr int NVAL = 10;
+constexpr uint32_t PART_BYTES = NMATH * NVAL * BATCH * 4;
+constexpr uint32_t PBLK_BYTES = PART_BYTES + NMATH * (BATCH / 32) * 4;
+
 // Second phase of the backward: lanes = (slot, part).  Each lane sums, over its SLOTS pixel pairs (pixel A = (x, y),
 // pixel B = (x, y+4) of first-phase lane 8y+x), the queued (G*dL/dalpha, alpha*T) of its slot against pixel-local
-// coordinates and the per-pixel upstream gradients; the parts are then added with shfl.xor.
+// coordinates and the per-pixel upstream gradients; the parts are then added with shfl.xor and the ten sums of each
+// slot are stored, without atomics, into the warp's row of the stage's partial block (a warp visits a record at most
+// once per stage).
 template <int SLOTS>
 __device__ __noinline__ void flush_queue(uint32_t q_base, uint32_t coef_base, uint32_t slot_base, int nq, int lane,
-                                         float Xc, float Yc, const uint32_t* __restrict__ tile_list,
-                                         const SplatRec* __restrict__ recs, SplatGrad* __restrict__ sg) {
+                                         float Xc, float Yc, uint32_t s_stage, uint32_t s_part) {
     using Q = QGeom<SLOTS>;
     const int slot = lane & (SLOTS - 1), part = lane / SLOTS;
-    // a slot remembers only the list position of its splat (one 4 B store per visit by lane 0): the id comes from the
-    // tile's list and mean2D / opacity from the splat's record here -- L2 hits issued before the sums, so their latency
-    // hides behind them
-    uint32_t gid = 0u;
+    // a slot remembers only the record index of its splat in the stage (one 4 B store per visit by lane 0); mean2D and
+    // opacity come from the record, which stays in the ring until the warp releases the stage
+    uint32_t rec = 0u;
     float4 si = make_float4(0.f, 0.f, 0.f, 0.f);                // mean2D.x, mean2D.y, -, opacity
     if (slot < nq) {
-        uint32_t pos;
-        asm volatile("ld.shared.u32 %0, [%1];" : "=r"(pos) : "r"(slot_base + slot * 4));
-        gid = __ldg(tile_list + pos);
-        const float4 g = __ldg(&recs[gid].g), c = __ldg(&recs[gid].c);
-        si = make_float4(g.x, g.y, 0.f, c.w);
+        rec = ldsu32(slot_base + slot * 4);
+        const float4 g = lds128(s_stage + rec * REC_BYTES);
+        si = make_float4(g.x, g.y, 0.f, lds32(s_stage + rec * REC_BYTES + 28));
     }
     const uint32_t qg = q_base + slot * 8 + part * SLOTS * Q::ROW, qd = qg + 32 * Q::ROW;
     const uint32_t ca = coef_base + part * SLOTS * 32;
@@ -512,24 +527,54 @@ __device__ __noinline__ void flush_queue(uint32_t q_base, uint32_t coef_base, ui
 #undef XADD
     }
     if (slot < nq) {
-        double* dst = reinterpret_cast<double*>(sg + gid);
         // pixel = centre + L, d = mean2D - pixel = u - L with u = mean2D - centre
         const float u = si.x - Xc, v = si.y - Yc, o = si.w;
-        // the ten sums of the splat = the three double4 of its SplatGrad record (ten fp64 reds per (quadrant, splat)),
-        // shared between the parts of the slot
-        const float4 qg = make_float4(o * (u * M0 - M1),                                   // sum w dx
-                                      o * (v * M0 - My),                                   // sum w dy
-                                      Cd, 0.f);                                            // dL/ddepth
-        const float4 qc = make_float4(o * (fmaf(u, fmaf(u, M0, -2.f * M1), M2)),           // sum w dx dx
-                                      o * (fmaf(u, fmaf(v, M0, -My), fmaf(-v, M1, Mxy))),  // sum w dx dy
-                                      o * (fmaf(v, fmaf(v, M0, -2.f * My), Myy)),          // sum w dy dy
-                                      M0);                                                 // dL/dopacity (sum G dL/dalpha)
-        const float4 qk = make_float4(Cr, Cg, Cb, 0.f);                                    // dL/drgb
-        if (Q::PARTS == 2) {
-            red_add_d4(dst + (part == 0 ? 0 : 8), part == 0 ? qg : qk, 3);
-            if (part == 0) red_add_d4(dst + 4, qc, 4);
-        } else {
-            if (part < 3) red_add_d4(dst + 4 * part, part == 0 ? qg : (part == 1 ? qc : qk), part == 1 ? 4 : 3);
+        // the ten sums of the splat, in the order of the non-padding doubles of its SplatGrad record
+        const float val[NVAL] = {o * (u * M0 - M1),                                   // sum w dx
+                                 o * (v * M0 - My),                                   // sum w dy
+                                 Cd,                                                  // dL/ddepth
+                                 o * (fmaf(u, fmaf(u, M0, -2.f * M1), M2)),           // sum w dx dx
+                                 o * (fmaf(u, fmaf(v, M0, -My), fmaf(-v, M1, Mxy))),  // sum w dx dy
+                                 o * (fmaf(v, fmaf(v, M0, -2.f * My), Myy)),          // sum w dy dy
+                                 M0,                                                  // dL/dopacity (sum G dL/dalpha)
+                                 Cr, Cg, Cb};                                         // dL/drgb
+        // every part of the slot holds all ten sums: each stores every PARTS-th of them
+#pragma unroll
+        for (int k = 0; k < NVAL; k++)
+            if (k % Q::PARTS == part) sts32(s_part + (k * BATCH + rec) * 4, val[k]);
+    }
+}
+
+// The stage's splats leave the CTA here, run by the last warp to release the stage; lanes = records.  Per record hit
+// by any quadrant, the partials of the warps that hit it are converted to fp64 and added in warp order 0, 1, 2, 3, then
+// ONE set of ten fp64 reds goes to its SplatGrad record (sm_90 has no vector fp64 red).  A sum of up to four fp32 values
+// in fp64 is exact unless their exponents lie more than 29 bits apart, so SplatGrad receives, to fp64 rounding, what
+// one set of reds per (quadrant, splat) would add -- with one set per (tile, splat) instead.
+__device__ __noinline__ void combine_stage(uint32_t s_blk, int lane, const uint32_t* __restrict__ list,
+                                           SplatGrad* __restrict__ sg) {
+    uint32_t hit[BATCH / 32], gid[BATCH / 32];
+#pragma unroll
+    for (int i = 0; i < BATCH / 32; i++) {              // bit w of hit[i]: warp w holds a partial of record i*32 + lane
+        uint32_t h = 0u;
+#pragma unroll
+        for (int w = 0; w < NMATH; w++) h |= ((ldsu32(s_blk + PART_BYTES + (w * (BATCH / 32) + i) * 4) >> lane) & 1u) << w;
+        hit[i] = h;
+        gid[i] = h ? __ldg(list + i * 32 + lane) : 0u;
+    }
+#pragma unroll
+    for (int i = 0; i < BATCH / 32; i++) {
+        if (!hit[i]) continue;
+        double* dst = reinterpret_cast<double*>(sg + gid[i]);
+        const uint32_t pa = s_blk + (i * 32 + lane) * 4;
+#pragma unroll
+        for (int k = 0; k < NVAL; k++) {
+            double s = 0.0;
+#pragma unroll
+            for (int w = 0; w < NMATH; w++) {           // absent partials are stale words: selected away, never added
+                const float p = lds32(pa + (w * NVAL + k) * BATCH * 4);
+                s += ((hit[i] >> w) & 1u) ? (double)p : 0.0;
+            }
+            atomicAdd(dst + (k < 3 ? k : k + 1), s);     // skips the padding double after dL/ddepth
         }
     }
 }
@@ -580,21 +625,25 @@ __device__ __forceinline__ void bwd_back(const BwdFront& f, u64& T2, u64& behind
     sts64(qd, lo(dchan), hi(dchan));
 }
 
-// PAIR: every loop iteration runs BOTH visits; when the group has an odd number of hits the second one is masked off
+// Every loop iteration runs BOTH visits; when the group has an odd number of hits the second one is masked off
 // (alpha = G = 0: T, behind and the queued values are then unchanged / zero, and its queue slot is not consumed) and the
 // queue is checked once per iteration (flushed early at SLOTS - 1) -- one branch region per iteration instead of three.
-template <int STAGES, int SLOTS, int MINB, bool VOTE, bool TMA, bool PAIR>
+// PBLK partial blocks: iteration `it` uses block it % PBLK (see the release below for why STAGES or STAGES + 1 is safe).
+template <int STAGES, int SLOTS, int PBLK, int MINB>
 __global__ void __launch_bounds__(NTHREADS, MINB)
 composite_backward_kernel(ViewArgs va, const SplatRec* __restrict__ recs, const uint32_t* __restrict__ point_list,
                           const uint32_t* __restrict__ ranges, const uint32_t* __restrict__ n_contrib,
                           const float* __restrict__ final_T, const float* __restrict__ dL_dcolor,
                           const float* __restrict__ dL_ddepth, const float* __restrict__ dL_dalpha,
                           SplatGrad* __restrict__ sg) {
+    static_assert(PBLK == STAGES || PBLK == STAGES + 1, "a partial block must outlive its stage's combine");
     using Q = QGeom<SLOTS>;
-    // dynamic shared memory: ring | queue | per-pixel upstream gradients | slot info | barriers | counters | wmax
+    // dynamic shared memory: ring | partial blocks | queue | per-pixel upstream gradients | slot info | barriers |
+    // counters | wmax
     extern __shared__ __align__(128) unsigned char smem[];
     const uint32_t s_rec = (uint32_t)__cvta_generic_to_shared(smem);
-    const uint32_t s_q = s_rec + STAGES * STAGE_BYTES;
+    const uint32_t s_part = s_rec + STAGES * STAGE_BYTES;
+    const uint32_t s_q = s_part + PBLK * PBLK_BYTES;
     const uint32_t s_coef = s_q + NMATH * Q::WARP;
     const uint32_t s_slot = s_coef + NMATH * 64 * 16;
     const uint32_t a_full = s_slot + NMATH * SLOTS * 4;
@@ -616,7 +665,7 @@ composite_backward_kernel(ViewArgs va, const SplatRec* __restrict__ recs, const 
     for (int o = 16; o > 0; o >>= 1) wmax = max(wmax, __shfl_xor_sync(0xFFFFFFFFu, wmax, o));
     if (lane == 0) s_wmax[warp] = wmax;
     if (tid == 0) {
-        for (int i = 0; i < STAGES; i++) { mbar_init(a_full + 8 * i, full_count(TMA)); s_cnt[i] = 0; }
+        for (int i = 0; i < STAGES; i++) { mbar_init(a_full + 8 * i, full_count(false)); s_cnt[i] = 0; }
         mbar_fence_init();
     }
     __syncthreads();
@@ -627,8 +676,8 @@ composite_backward_kernel(ViewArgs va, const SplatRec* __restrict__ recs, const 
     // stages are gathered from the back of the list: iteration `it` holds list positions [(nb-1-it)*BATCH, +BATCH)
     auto produce = [&](int it, uint32_t stage) {
         const int base = (nb - 1 - it) * BATCH;
-        produce_stage<false, TMA>(recs, point_list + start + base, min(BATCH, (int)nproc - base), s_rec + stage * STAGE_BYTES,
-                             0u, a_full + 8 * stage, lane);
+        produce_stage<false, false>(recs, point_list + start + base, min(BATCH, (int)nproc - base), s_rec + stage * STAGE_BYTES,
+                                    0u, a_full + 8 * stage, lane);
     };
     if (warp < STAGES && warp < nb) produce(warp, warp);       // first fill; afterwards the last warp to finish a stage refills it
 
@@ -663,53 +712,48 @@ composite_backward_kernel(ViewArgs va, const SplatRec* __restrict__ recs, const 
     for (int it = 0; it < nb; it++) {
         mbar_wait(a_full + 8 * rs.stage, rs.phase);
         const int base = (nb - 1 - it) * BATCH;
+        const uint32_t sr = s_rec + rs.stage * STAGE_BYTES;
+        const uint32_t blk = s_part + (uint32_t)(it % PBLK) * PBLK_BYTES;
+        const uint32_t s_pw = blk + warp * NVAL * BATCH * 4;          // this warp's rows of the partial block
         if ((uint32_t)base < wmax) {                      // otherwise the whole stage is past this warp's last contributor
             const int n = min(BATCH, (int)nproc - base);
-            const uint32_t sr = s_rec + rs.stage * STAGE_BYTES;
             uint32_t m[BATCH / 32];
             stage_masks(sr, n, lane, X0f, Y0f, m);
+            if (lane == 0)
+                asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(blk + PART_BYTES + warp * 16), "r"(m[0]), "r"(m[1]),
+                             "r"(m[2]), "r"(m[3]) : "memory");
 #pragma unroll
             for (int i = BATCH / 32 - 1; i >= 0; i--) {
                 uint32_t bal = m[i];
-                const uint32_t rg = sr + i * 32 * REC_BYTES, pos0 = (uint32_t)(base + i * 32);
+                const uint32_t rg = sr + i * 32 * REC_BYTES, r0 = (uint32_t)(i * 32), pos0 = (uint32_t)base + r0;
                 // two visits per iteration, from the back: everything but the T / behind recurrences and the queue slot is
                 // independent between them (bwd_front), so the two instruction streams interleave
                 while (bal) {
-                    if (PAIR && nq > SLOTS - 2) { __syncwarp(); flush_queue<SLOTS>(q_base, coef_base, slot_base, nq, lane, Xc, Yc, tile_list, recs, sg); __syncwarp(); nq = 0; }
+                    if (nq > SLOTS - 2) { __syncwarp(); flush_queue<SLOTS>(q_base, coef_base, slot_base, nq, lane, Xc, Yc, sr, s_pw); __syncwarp(); nq = 0; }
                     const int j0 = hibit(bal);
                     const uint32_t b0 = 1u << j0;
                     bal &= ~b0;
                     const bool two = bal != 0;
                     const int j1 = hibit(two ? bal : b0);        // (a select on the mask, not a branch around the bfind)
                     bal &= ~(1u << j1);
-                    if (PAIR) {
-                        const BwdFront g0 = bwd_front(rg + j0 * REC_BYTES, pos0 + j0, pxf, py2, lcA, lcB, gC0, gC1, gC2, gD, gA, bgT);
-                        const BwdFront g1 = bwd_front(rg + j1 * REC_BYTES, pos0 + j1, pxf, py2, lcA, lcB, gC0, gC1, gC2, gD, gA, bgT, two);
-                        bwd_back(g0, T2, behind, qwG + nq * 8, qwD + nq * 8);
-                        bwd_back(g1, T2, behind, qwG + nq * 8 + 8, qwD + nq * 8 + 8);
-                        if (lane == 0) {
-                            asm volatile("st.shared.u32 [%0], %1;" ::"r"(slot_base + nq * 4), "r"(pos0 + j0) : "memory");
-                            asm volatile("st.shared.u32 [%0+4], %1;" ::"r"(slot_base + nq * 4), "r"(pos0 + j1) : "memory");
-                        }
-                        nq += two ? 2 : 1;
-                        continue;
+                    const BwdFront g0 = bwd_front(rg + j0 * REC_BYTES, pos0 + j0, pxf, py2, lcA, lcB, gC0, gC1, gC2, gD, gA, bgT);
+                    const BwdFront g1 = bwd_front(rg + j1 * REC_BYTES, pos0 + j1, pxf, py2, lcA, lcB, gC0, gC1, gC2, gD, gA, bgT, two);
+                    bwd_back(g0, T2, behind, qwG + nq * 8, qwD + nq * 8);
+                    bwd_back(g1, T2, behind, qwG + nq * 8 + 8, qwD + nq * 8 + 8);
+                    if (lane == 0) {
+                        asm volatile("st.shared.u32 [%0], %1;" ::"r"(slot_base + nq * 4), "r"(r0 + j0) : "memory");
+                        asm volatile("st.shared.u32 [%0+4], %1;" ::"r"(slot_base + nq * 4), "r"(r0 + j1) : "memory");
                     }
-                    const BwdFront f0 = bwd_front(rg + j0 * REC_BYTES, pos0 + j0, pxf, py2, lcA, lcB, gC0, gC1, gC2, gD, gA, bgT);
-                    const BwdFront f1 = bwd_front(rg + j1 * REC_BYTES, pos0 + j1, pxf, py2, lcA, lcB, gC0, gC1, gC2, gD, gA, bgT);
-                    if (!VOTE || __any_sync(0xFFFFFFFFu, f0.any)) {
-                        bwd_back(f0, T2, behind, qwG + nq * 8, qwD + nq * 8);
-                        if (lane == 0) asm volatile("st.shared.u32 [%0], %1;" ::"r"(slot_base + nq * 4), "r"(pos0 + j0) : "memory");
-                        if (++nq == SLOTS) { __syncwarp(); flush_queue<SLOTS>(q_base, coef_base, slot_base, SLOTS, lane, Xc, Yc, tile_list, recs, sg); __syncwarp(); nq = 0; }
-                    }
-                    if (two && (!VOTE || __any_sync(0xFFFFFFFFu, f1.any))) {
-                        bwd_back(f1, T2, behind, qwG + nq * 8, qwD + nq * 8);
-                        if (lane == 0) asm volatile("st.shared.u32 [%0], %1;" ::"r"(slot_base + nq * 4), "r"(pos0 + j1) : "memory");
-                        if (++nq == SLOTS) { __syncwarp(); flush_queue<SLOTS>(q_base, coef_base, slot_base, SLOTS, lane, Xc, Yc, tile_list, recs, sg); __syncwarp(); nq = 0; }
-                    }
+                    nq += two ? 2 : 1;
                 }
             }
+            // every visit of the stage is flushed before the stage is released, so its partial block is complete once
+            // all four warps have released it
+            if (nq > 0) { __syncwarp(); flush_queue<SLOTS>(q_base, coef_base, slot_base, nq, lane, Xc, Yc, sr, s_pw); nq = 0; }
+        } else if (lane == 0) {
+            asm volatile("st.shared.v4.u32 [%0], {%1,%1,%1,%1};" ::"r"(blk + PART_BYTES + warp * 16), "r"(0u) : "memory");
         }
-        // release the stage; the last of the four warps to do so refills it
+        // release the stage; the last of the four warps to do so combines its partial block and refills it
         __syncwarp();
         uint32_t tot = 0;
         if (lane == 0) { __threadfence_block(); tot = atomicAdd(&s_cnt[rs.stage], 1u) + 1u; }
@@ -717,22 +761,24 @@ composite_backward_kernel(ViewArgs va, const SplatRec* __restrict__ recs, const 
         if (tot == NMATH) {
             if (lane == 0) { __threadfence_block(); s_cnt[rs.stage] = 0; }       // acquire side of the stage hand-over
             __syncwarp();
+            // Block it % PBLK is next written in iteration it + PBLK.  PBLK == STAGES: that iteration's records arrive
+            // through the refill below, so the combine runs before it.  PBLK == STAGES + 1: iteration it + PBLK arrives
+            // through the refill issued when iteration it + 1 is released by all four warps, this one included, and this
+            // warp releases it only after the combine.
+            if (PBLK == STAGES) combine_stage(blk, lane, tile_list + base, sg);
             if (it + STAGES < nb) {
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // the stage was read through the generic proxy
                 produce(it + STAGES, rs.stage);
             }
+            if (PBLK != STAGES) combine_stage(blk, lane, tile_list + base, sg);
         }
         rs.advance(STAGES);
     }
-    if (nq > 0) {
-        __syncwarp();
-        flush_queue<SLOTS>(q_base, coef_base, slot_base, nq, lane, Xc, Yc, tile_list, recs, sg);
-    }
 }
 
-constexpr size_t bwd_smem_bytes(int stages, int slots) {
-    return (size_t)stages * STAGE_BYTES + NMATH * 64 * (size_t)(slots + 1) * 8 + NMATH * 64 * 16 + NMATH * (size_t)slots * 4 +
-           8 * (size_t)stages + 4 * (size_t)stages + 16;
+constexpr size_t bwd_smem_bytes(int stages, int slots, int pblk) {
+    return (size_t)stages * STAGE_BYTES + (size_t)pblk * PBLK_BYTES + NMATH * 64 * (size_t)(slots + 1) * 8 + NMATH * 64 * 16 +
+           NMATH * (size_t)slots * 4 + 8 * (size_t)stages + 4 * (size_t)stages + 16;
 }
 
 bool gather_tma() {       // GS_B200_GATHER=tma selects the TMA bulk-copy gather instead of the cp.async default
@@ -792,21 +838,17 @@ int gs_launch_render_backward(const ViewArgs& va, const SplatRec* recs, const ui
                               SplatGrad* sg, cudaStream_t s) {
     if (use_r1()) return gs_launch_render_backward_r1(va, recs, point_list, ranges, n_contrib, final_T, dL_dcolor, dL_ddepth, dL_dalpha, sg, s);
     dim3 grid(va.tiles_x, va.tiles_y);
-    // Selectable: ring depth (GS_B200_BWD_STAGES 2/3) and the TMA gather (GS_B200_GATHER=tma).
-    static const int stages = env_int("GS_B200_BWD_STAGES", 2);
-    static const bool pair = env_int("GS_B200_BWD_PAIR", 1) != 0;      // both visits of an iteration unconditional (second masked)
-#define BWD(ST, TM, PR)                                                                                                    \
-    do {                                                                                                                   \
-        static const cudaError_t attr = cudaFuncSetAttribute(composite_backward_kernel<ST, 16, 4, false, TM, PR>,          \
-                                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bwd_smem_bytes(ST, 16)); \
-        GS_CUDA_CHECK(attr);                                                                                               \
-        composite_backward_kernel<ST, 16, 4, false, TM, PR><<<grid, NTHREADS, bwd_smem_bytes(ST, 16), s>>>(va, recs, point_list, ranges, n_contrib, final_T, dL_dcolor, dL_ddepth, dL_dalpha, sg); \
-    } while (0)
-    if (gather_tma()) BWD(2, true, false);
-    else if (stages == 3) BWD(3, false, false);
-    else if (pair) BWD(2, false, true);
-    else BWD(2, false, false);
-#undef BWD
+    // ring depth, queued visits per flush, partial blocks, CTAs per SM: 2 x 6 KB ring + 2 x 20 KB partial blocks + 34 KB
+    // queue = 92 KB, two CTAs per SM.  Measured on an H100 SXM against 8 visits per flush (75 KB, three CTAs per SM; the
+    // moments' fp32 summation order then changes too), a third ring stage, and a third partial block with the refill
+    // issued before the combine: all slower.
+    constexpr int ST = 2, SL = 16, PB = 2, MB = 2;
+    constexpr size_t smem = bwd_smem_bytes(ST, SL, PB);
+    static const cudaError_t attr = cudaFuncSetAttribute(composite_backward_kernel<ST, SL, PB, MB>,
+                                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    GS_CUDA_CHECK(attr);
+    composite_backward_kernel<ST, SL, PB, MB><<<grid, NTHREADS, smem, s>>>(va, recs, point_list, ranges, n_contrib, final_T,
+                                                                          dL_dcolor, dL_ddepth, dL_dalpha, sg);
     gs_count_launches(1);
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
