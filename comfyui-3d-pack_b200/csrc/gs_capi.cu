@@ -605,7 +605,6 @@ int step_core(int V, int H, int W, int sh_degree, float scale_modifier, const fl
     auto enqueue_pre = [&](int k) -> int {           // batched preprocess of chunk k on the aux stream
         const int v0 = k * VB, nv = std::min(VB, V - v0);
         const WS& w = ws[k & (nsets - 1)];
-        if (!O.forward_only) GS_CUDA_CHECK(cudaMemsetAsync(w.sg, 0, (size_t)nv * N * sizeof(SplatGrad), aux));
         GS_CUDA_CHECK(cudaMemsetAsync(w.minkeys, 0xFF, 256 * 4, aux));
         { StageTimer t(0, aux);
         if (gs_launch_preprocess_multi(views_dev + (size_t)v0 * 40, nv, W, H, sh_degree, scale_modifier, N, M, par.means,
@@ -648,6 +647,11 @@ int step_core(int V, int H, int W, int sh_degree, float scale_modifier, const fl
             if (fwd_phase_a(*ctx[q], &vw, N, M, par.means, par.shs, par.colors, par.opac, par.scales, par.rots, nullptr,
                             img, img + 3 * npix, img + 4 * npix, w.radii + o, &st[q], S.host_total, &pre)) return 1;
             GS_CUDA_CHECK(cudaEventRecord(S.evA, S.stream));
+            // The view's SplatGrad slice is zeroed here, on its slot stream, so the write overlaps the other slot's
+            // composites instead of delaying the batched preprocess.  Also for a view without pairs, whose composite
+            // backward is skipped: the batched preprocess-backward reads the slice for every Gaussian with radii > 0.
+            // (Placed after evA, so the host's wait for the pair count does not wait for it too.)
+            if (!O.forward_only) GS_CUDA_CHECK(cudaMemsetAsync(w.sg + o, 0, (size_t)N * sizeof(SplatGrad), S.stream));
             return S.failed ? 1 : 0;
         };
 

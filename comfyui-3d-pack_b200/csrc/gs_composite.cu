@@ -121,6 +121,11 @@ __device__ __forceinline__ uint32_t ldsu32(uint32_t addr) {
 __device__ __forceinline__ void sts32(uint32_t addr, float a) {
     asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(a) : "memory");
 }
+// fp64 add to global memory that returns nothing.  atomicAdd(double*) with its result unused compiles to a returning
+// ATOMG inside combine_stage, and the warp then waits for each reply; red.global compiles to REDG, which it does not.
+__device__ __forceinline__ void red_add_f64(double* p, double v) {
+    asm volatile("red.global.add.f64 [%0], %1;" ::"l"(p), "d"(v) : "memory");
+}
 __device__ __forceinline__ uint32_t ld_volatile_s32(uint32_t addr) {
     uint32_t v;
     asm volatile("ld.volatile.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
@@ -574,7 +579,7 @@ __device__ __noinline__ void combine_stage(uint32_t s_blk, int lane, const uint3
                 const float p = lds32(pa + (w * NVAL + k) * BATCH * 4);
                 s += ((hit[i] >> w) & 1u) ? (double)p : 0.0;
             }
-            atomicAdd(dst + (k < 3 ? k : k + 1), s);     // skips the padding double after dL/ddepth
+            red_add_f64(dst + (k < 3 ? k : k + 1), s);   // skips the padding double after dL/ddepth
         }
     }
 }
