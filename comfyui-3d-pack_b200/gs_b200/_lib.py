@@ -140,9 +140,16 @@ lib.ngp_b200_mlp2_fwd.restype = _I
 lib.ngp_b200_mlp2_fwd.argtypes = [_P, _L, _I, _I, _I, _P, _P, _P, _P]
 lib.ngp_b200_mlp2_bwd.restype = _I
 lib.ngp_b200_mlp2_bwd.argtypes = [_P, _L, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P]
+lib.ngp_b200_mcubes_scratch_bytes.restype = C.c_size_t
+lib.ngp_b200_mcubes_scratch_bytes.argtypes = [_I, _I, _I]
+lib.ngp_b200_mcubes_count.restype = _I
+lib.ngp_b200_mcubes_count.argtypes = [_P, _I, _I, _I, _F, _P, _P, _P]
+lib.ngp_b200_mcubes_write.restype = _I
+lib.ngp_b200_mcubes_write.argtypes = [_P, _I, _I, _I, _F, C.POINTER(C.c_ulonglong), _P, _P, _P, _P]
 NGP_EXPORTS = ["ngp_b200_mlp2_supported", "ngp_b200_mlp2_fwd", "ngp_b200_mlp2_bwd","ngp_b200_grid_encode_fwd", "ngp_b200_grid_encode_bwd", "ngp_b200_grid_tv_grad", "ngp_b200_march_scratch_bytes",
                "ngp_b200_march_count", "ngp_b200_march_write", "ngp_b200_ray_ranges", "ngp_b200_weights_fwd",
-               "ngp_b200_weights_bwd", "ngp_b200_accumulate_fwd", "ngp_b200_accumulate_bwd"]
+               "ngp_b200_weights_bwd", "ngp_b200_accumulate_fwd", "ngp_b200_accumulate_bwd",
+               "ngp_b200_mcubes_scratch_bytes", "ngp_b200_mcubes_count", "ngp_b200_mcubes_write"]
 
 lib.gs_b200_activate.restype = _I
 lib.gs_b200_activate.argtypes = [_I, _P, _P, _P, _P, _P, _P, _P]

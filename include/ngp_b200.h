@@ -65,6 +65,21 @@ int32_t ngp_b200_mlp2_fwd(const float* X, int64_t N, int32_t Din, int32_t H, int
                           float* Y, void* stream);
 int32_t ngp_b200_mlp2_bwd(const float* X, int64_t N, int32_t Din, int32_t H, int32_t Dout, const float* W1, const float* W2,
                           const float* GY, float* GX, float* GW1, float* GW2, void* stream);
+
+/* ---- marching cubes (PyMCubes marching_cubes(volume, iso); mesh_processer/mesh_utils.py:509, LGM
+ * nerf_marching_cubes_converter.py:245) ---------------------------------------------------------------------
+ * volume[X,Y,Z] fp32 C-contiguous; a corner is above iff value > iso.  Two phases: count -> (host copies totals_dev3)
+ * -> write.  totals = {vertices, triangles, non-finite flag}.  verts[V,3] fp32: column c is the coordinate along array
+ * axis c, in index units; tris[F,3] int32, counter-clockwise seen from the below-iso side.  Vertices are ordered by
+ * (owner grid point, axis), triangles by (cell, case-table order).  A dimension < 2 gives V = F = 0.  write fails,
+ * before writing anything, on a non-finite sample or when V or F reaches 2^31.  scratch >= mcubes_scratch_bytes and
+ * is passed unchanged from count to write. */
+size_t ngp_b200_mcubes_scratch_bytes(int32_t X, int32_t Y, int32_t Z);
+int32_t ngp_b200_mcubes_count(const float* volume, int32_t X, int32_t Y, int32_t Z, float iso,
+                              unsigned long long* totals_dev3, void* scratch, void* stream);
+int32_t ngp_b200_mcubes_write(const float* volume, int32_t X, int32_t Y, int32_t Z, float iso,
+                              const unsigned long long* totals_host3, float* verts, int32_t* tris, void* scratch,
+                              void* stream);
 #ifdef __cplusplus
 }
 #endif
