@@ -473,21 +473,23 @@ template <int SLOTS> struct QGeom {
     static constexpr int PARTS = 32 / SLOTS;       // lanes = (slot, part); a part owns SLOTS consecutive lane rows
 };
 
-// Partial block of one ring stage: the ten per-splat sums of every (warp, record) the warp visited, fp32,
-// [warp][value][record] (value-major, so the combine's lanes = records read consecutive words), followed by the warps'
-// hit masks of the stage [warp][BATCH / 32], which say which partials exist (the block is never cleared).
+// Partial block: the ten per-splat sums of every (warp, record) the warp visited in one stage, fp32,
+// [warp][value][record] (value-major, so the combine's lanes = records read consecutive words).  ONE block serves both
+// ring stages (see the gate in composite_backward_kernel).  Each ring stage has its own hit-mask block
+// [warp][BATCH / 32], which says which partials exist (the partial block is never cleared).
 constexpr int NVAL = 10;
 constexpr uint32_t PART_BYTES = NMATH * NVAL * BATCH * 4;
-constexpr uint32_t PBLK_BYTES = PART_BYTES + NMATH * (BATCH / 32) * 4;
+constexpr uint32_t MASK_BYTES = NMATH * (BATCH / 32) * 4;
 
 // Second phase of the backward: lanes = (slot, part).  Each lane sums, over its SLOTS pixel pairs (pixel A = (x, y),
 // pixel B = (x, y+4) of first-phase lane 8y+x), the queued (G*dL/dalpha, alpha*T) of its slot against pixel-local
 // coordinates and the per-pixel upstream gradients; the parts are then added with shfl.xor and the ten sums of each
-// slot are stored, without atomics, into the warp's row of the stage's partial block (a warp visits a record at most
-// once per stage).
+// slot are stored, without atomics, into the warp's row of the partial block (a warp visits a record at most once per
+// stage).  Those stores wait until the block is free: phase `free_parity` of the mbarrier `free_bar` has completed.
 template <int SLOTS>
 __device__ __noinline__ void flush_queue(uint32_t q_base, uint32_t coef_base, uint32_t slot_base, int nq, int lane,
-                                         float Xc, float Yc, uint32_t s_stage, uint32_t s_part) {
+                                         float Xc, float Yc, uint32_t s_stage, uint32_t s_part, uint32_t free_bar,
+                                         uint32_t free_parity) {
     using Q = QGeom<SLOTS>;
     const int slot = lane & (SLOTS - 1), part = lane / SLOTS;
     // a slot remembers only the record index of its splat in the stage (one 4 B store per visit by lane 0); mean2D and
@@ -531,6 +533,7 @@ __device__ __noinline__ void flush_queue(uint32_t q_base, uint32_t coef_base, ui
         XADD(M0); XADD(M1); XADD(M2); XADD(My); XADD(Mxy); XADD(Myy); XADD(Cd); XADD(Cr); XADD(Cg); XADD(Cb);
 #undef XADD
     }
+    mbar_wait(free_bar, free_parity);
     if (slot < nq) {
         // pixel = centre + L, d = mean2D - pixel = u - L with u = mean2D - centre
         const float u = si.x - Xc, v = si.y - Yc, o = si.w;
@@ -555,14 +558,14 @@ __device__ __noinline__ void flush_queue(uint32_t q_base, uint32_t coef_base, ui
 // ONE set of ten fp64 reds goes to its SplatGrad record (sm_90 has no vector fp64 red).  A sum of up to four fp32 values
 // in fp64 is exact unless their exponents lie more than 29 bits apart, so SplatGrad receives, to fp64 rounding, what
 // one set of reds per (quadrant, splat) would add -- with one set per (tile, splat) instead.
-__device__ __noinline__ void combine_stage(uint32_t s_blk, int lane, const uint32_t* __restrict__ list,
+__device__ __noinline__ void combine_stage(uint32_t s_part, uint32_t s_mask, int lane, const uint32_t* __restrict__ list,
                                            SplatGrad* __restrict__ sg) {
     uint32_t hit[BATCH / 32], gid[BATCH / 32];
 #pragma unroll
     for (int i = 0; i < BATCH / 32; i++) {              // bit w of hit[i]: warp w holds a partial of record i*32 + lane
         uint32_t h = 0u;
 #pragma unroll
-        for (int w = 0; w < NMATH; w++) h |= ((ldsu32(s_blk + PART_BYTES + (w * (BATCH / 32) + i) * 4) >> lane) & 1u) << w;
+        for (int w = 0; w < NMATH; w++) h |= ((ldsu32(s_mask + (w * (BATCH / 32) + i) * 4) >> lane) & 1u) << w;
         hit[i] = h;
         gid[i] = h ? __ldg(list + i * 32 + lane) : 0u;
     }
@@ -570,7 +573,7 @@ __device__ __noinline__ void combine_stage(uint32_t s_blk, int lane, const uint3
     for (int i = 0; i < BATCH / 32; i++) {
         if (!hit[i]) continue;
         double* dst = reinterpret_cast<double*>(sg + gid[i]);
-        const uint32_t pa = s_blk + (i * 32 + lane) * 4;
+        const uint32_t pa = s_part + (i * 32 + lane) * 4;
 #pragma unroll
         for (int k = 0; k < NVAL; k++) {
             double s = 0.0;
@@ -633,26 +636,37 @@ __device__ __forceinline__ void bwd_back(const BwdFront& f, u64& T2, u64& behind
 // Every loop iteration runs BOTH visits; when the group has an odd number of hits the second one is masked off
 // (alpha = G = 0: T, behind and the queued values are then unchanged / zero, and its queue slot is not consumed) and the
 // queue is checked once per iteration (flushed early at SLOTS - 1) -- one branch region per iteration instead of three.
-// PBLK partial blocks: iteration `it` uses block it % PBLK (see the release below for why STAGES or STAGES + 1 is safe).
-template <int STAGES, int SLOTS, int PBLK, int MINB>
+//
+// One partial block serves every iteration, behind a gate: the mbarrier a_free completes phase `it` when the combine of
+// iteration `it` has read the block, and flush_queue waits for phase it - 1 before it stores partials of iteration
+// `it`.  A warp waits there only when it has partials to store, so a warp that runs ahead still computes its stage
+// masks, its first-phase visits and the second-phase sums of its first flush before it blocks.  No deadlock: a waiting
+// warp in iteration `it` has released stage it - 1, so the last warp to release it, which runs that combine, is not
+// among the waiters; and the warps still in iteration it - 1 wait (if at all) for the combine of it - 2, which has
+// completed, because stage `it` was refilled after it.  That also bounds the phases in flight: when a warp enters
+// iteration `it`, at most the combine of it - 1 is pending (the refill of a stage follows its combine), so the parity
+// wait cannot alias an older phase -- which holds for a ring of at most two stages.
+template <int STAGES, int SLOTS, int MINB>
 __global__ void __launch_bounds__(NTHREADS, MINB)
 composite_backward_kernel(ViewArgs va, const SplatRec* __restrict__ recs, const uint32_t* __restrict__ point_list,
                           const uint32_t* __restrict__ ranges, const uint32_t* __restrict__ n_contrib,
                           const float* __restrict__ final_T, const float* __restrict__ dL_dcolor,
                           const float* __restrict__ dL_ddepth, const float* __restrict__ dL_dalpha,
                           SplatGrad* __restrict__ sg) {
-    static_assert(PBLK == STAGES || PBLK == STAGES + 1, "a partial block must outlive its stage's combine");
+    static_assert(STAGES <= 2, "the partial-block gate waits on mbarrier parity: one combine in flight at most");
     using Q = QGeom<SLOTS>;
-    // dynamic shared memory: ring | partial blocks | queue | per-pixel upstream gradients | slot info | barriers |
-    // counters | wmax
+    // dynamic shared memory: ring | partial block | hit masks per stage | queue | per-pixel upstream gradients |
+    // slot info | barriers (full per stage, free) | counters | wmax
     extern __shared__ __align__(128) unsigned char smem[];
     const uint32_t s_rec = (uint32_t)__cvta_generic_to_shared(smem);
     const uint32_t s_part = s_rec + STAGES * STAGE_BYTES;
-    const uint32_t s_q = s_part + PBLK * PBLK_BYTES;
+    const uint32_t s_mask = s_part + PART_BYTES;
+    const uint32_t s_q = s_mask + STAGES * MASK_BYTES;
     const uint32_t s_coef = s_q + NMATH * Q::WARP;
     const uint32_t s_slot = s_coef + NMATH * 64 * 16;
     const uint32_t a_full = s_slot + NMATH * SLOTS * 4;
-    uint32_t* s_cnt = reinterpret_cast<uint32_t*>(smem + (a_full + 8 * STAGES - s_rec));
+    const uint32_t a_free = a_full + 8 * STAGES;
+    uint32_t* s_cnt = reinterpret_cast<uint32_t*>(smem + (a_free + 8 - s_rec));
     volatile uint32_t* s_wmax = s_cnt + STAGES;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int tile = blockIdx.y * va.tiles_x + blockIdx.x;
@@ -671,6 +685,7 @@ composite_backward_kernel(ViewArgs va, const SplatRec* __restrict__ recs, const 
     if (lane == 0) s_wmax[warp] = wmax;
     if (tid == 0) {
         for (int i = 0; i < STAGES; i++) { mbar_init(a_full + 8 * i, full_count(false)); s_cnt[i] = 0; }
+        mbar_init(a_free, 1);
         mbar_fence_init();
     }
     __syncthreads();
@@ -718,14 +733,18 @@ composite_backward_kernel(ViewArgs va, const SplatRec* __restrict__ recs, const 
         mbar_wait(a_full + 8 * rs.stage, rs.phase);
         const int base = (nb - 1 - it) * BATCH;
         const uint32_t sr = s_rec + rs.stage * STAGE_BYTES;
-        const uint32_t blk = s_part + (uint32_t)(it % PBLK) * PBLK_BYTES;
-        const uint32_t s_pw = blk + warp * NVAL * BATCH * 4;          // this warp's rows of the partial block
+        const uint32_t msk = s_mask + rs.stage * MASK_BYTES;
+        const uint32_t s_pw = s_part + warp * NVAL * BATCH * 4;      // this warp's rows of the partial block
+        // phase it - 1 of a_free: the combine of iteration it - 1 has read the block (for it = 0, parity 1 of a fresh
+        // mbarrier counts as complete)
+        const uint32_t free_par = (uint32_t)(it + 1) & 1u;
         if ((uint32_t)base < wmax) {                      // otherwise the whole stage is past this warp's last contributor
             const int n = min(BATCH, (int)nproc - base);
             uint32_t m[BATCH / 32];
             stage_masks(sr, n, lane, X0f, Y0f, m);
+            // the stage's own mask block: its last reader, the combine of iteration it - STAGES, ran before the refill
             if (lane == 0)
-                asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(blk + PART_BYTES + warp * 16), "r"(m[0]), "r"(m[1]),
+                asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(msk + warp * 16), "r"(m[0]), "r"(m[1]),
                              "r"(m[2]), "r"(m[3]) : "memory");
 #pragma unroll
             for (int i = BATCH / 32 - 1; i >= 0; i--) {
@@ -734,7 +753,7 @@ composite_backward_kernel(ViewArgs va, const SplatRec* __restrict__ recs, const 
                 // two visits per iteration, from the back: everything but the T / behind recurrences and the queue slot is
                 // independent between them (bwd_front), so the two instruction streams interleave
                 while (bal) {
-                    if (nq > SLOTS - 2) { __syncwarp(); flush_queue<SLOTS>(q_base, coef_base, slot_base, nq, lane, Xc, Yc, sr, s_pw); __syncwarp(); nq = 0; }
+                    if (nq > SLOTS - 2) { __syncwarp(); flush_queue<SLOTS>(q_base, coef_base, slot_base, nq, lane, Xc, Yc, sr, s_pw, a_free, free_par); __syncwarp(); nq = 0; }
                     const int j0 = hibit(bal);
                     const uint32_t b0 = 1u << j0;
                     bal &= ~b0;
@@ -752,13 +771,14 @@ composite_backward_kernel(ViewArgs va, const SplatRec* __restrict__ recs, const 
                     nq += two ? 2 : 1;
                 }
             }
-            // every visit of the stage is flushed before the stage is released, so its partial block is complete once
-            // all four warps have released it
-            if (nq > 0) { __syncwarp(); flush_queue<SLOTS>(q_base, coef_base, slot_base, nq, lane, Xc, Yc, sr, s_pw); nq = 0; }
+            // every visit of the stage is flushed before the stage is released, so the partial block holds the whole
+            // stage once all four warps have released it
+            if (nq > 0) { __syncwarp(); flush_queue<SLOTS>(q_base, coef_base, slot_base, nq, lane, Xc, Yc, sr, s_pw, a_free, free_par); nq = 0; }
         } else if (lane == 0) {
-            asm volatile("st.shared.v4.u32 [%0], {%1,%1,%1,%1};" ::"r"(blk + PART_BYTES + warp * 16), "r"(0u) : "memory");
+            asm volatile("st.shared.v4.u32 [%0], {%1,%1,%1,%1};" ::"r"(msk + warp * 16), "r"(0u) : "memory");
         }
-        // release the stage; the last of the four warps to do so combines its partial block and refills it
+        // release the stage; the last of the four warps to do so combines the partial block, frees it and refills the
+        // stage
         __syncwarp();
         uint32_t tot = 0;
         if (lane == 0) { __threadfence_block(); tot = atomicAdd(&s_cnt[rs.stage], 1u) + 1u; }
@@ -766,24 +786,44 @@ composite_backward_kernel(ViewArgs va, const SplatRec* __restrict__ recs, const 
         if (tot == NMATH) {
             if (lane == 0) { __threadfence_block(); s_cnt[rs.stage] = 0; }       // acquire side of the stage hand-over
             __syncwarp();
-            // Block it % PBLK is next written in iteration it + PBLK.  PBLK == STAGES: that iteration's records arrive
-            // through the refill below, so the combine runs before it.  PBLK == STAGES + 1: iteration it + PBLK arrives
-            // through the refill issued when iteration it + 1 is released by all four warps, this one included, and this
-            // warp releases it only after the combine.
-            if (PBLK == STAGES) combine_stage(blk, lane, tile_list + base, sg);
+            combine_stage(s_part, msk, lane, tile_list + base, sg);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(a_free);          // release: the combine's reads of the block precede later stores
+            // the refill comes after the combine: the stage's mask block is rewritten once its records arrive, and a warp
+            // can enter iteration it + STAGES only when the combine of iteration it is complete (see the gate above)
             if (it + STAGES < nb) {
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // the stage was read through the generic proxy
                 produce(it + STAGES, rs.stage);
             }
-            if (PBLK != STAGES) combine_stage(blk, lane, tile_list + base, sg);
         }
         rs.advance(STAGES);
     }
 }
 
-constexpr size_t bwd_smem_bytes(int stages, int slots, int pblk) {
-    return (size_t)stages * STAGE_BYTES + (size_t)pblk * PBLK_BYTES + NMATH * 64 * (size_t)(slots + 1) * 8 + NMATH * 64 * 16 +
-           NMATH * (size_t)slots * 4 + 8 * (size_t)stages + 4 * (size_t)stages + 16;
+constexpr size_t bwd_smem_bytes(int stages, int slots) {
+    return (size_t)stages * (STAGE_BYTES + MASK_BYTES) + PART_BYTES + NMATH * 64 * (size_t)(slots + 1) * 8 +
+           NMATH * 64 * 16 + NMATH * (size_t)slots * 4 + 8 * (size_t)stages + 8 + 4 * (size_t)stages + 16;
+}
+
+// The shipped backward: ring depth, queued visits per flush, CTAs per SM.  2 x 6 KB ring + 20 KB partial block + 34 KB
+// queue + 4 KB upstream gradients = 70.4 KB, three CTAs per SM (an H100 SM has 228 KB of shared memory and reserves
+// 1 KB per CTA).  Measured on an H100 against one partial block per stage (92.6 KB, two CTAs per SM): 0.654-0.661
+// against 0.739 ms per config-1 view.  A third ring stage would take 76.5 KB and fall back to two CTAs per SM.
+constexpr int BWD_STAGES = 2, BWD_SLOTS = 16, BWD_MINB = 3;
+constexpr size_t BWD_SMEM = bwd_smem_bytes(BWD_STAGES, BWD_SLOTS);
+static_assert(BWD_MINB * (BWD_SMEM + 1024) <= 228 * 1024, "the backward's shared memory must fit BWD_MINB CTAs per SM");
+#define BWD_KERNEL composite_backward_kernel<BWD_STAGES, BWD_SLOTS, BWD_MINB>
+
+// Dynamic shared memory beyond 48 KB must be allowed per kernel, and three CTAs of 70 KB need the largest shared-memory
+// carveout (228 KB) of the unified L1.  Set once, before the first launch or occupancy query.
+cudaError_t bwd_kernel_attributes() {
+    static const cudaError_t err = []() {
+        cudaError_t e = cudaFuncSetAttribute(BWD_KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM);
+        if (e == cudaSuccess)
+            e = cudaFuncSetAttribute(BWD_KERNEL, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        return e;
+    }();
+    return err;
 }
 
 bool gather_tma() {       // GS_B200_GATHER=tma selects the TMA bulk-copy gather instead of the cp.async default
@@ -843,18 +883,20 @@ int gs_launch_render_backward(const ViewArgs& va, const SplatRec* recs, const ui
                               SplatGrad* sg, cudaStream_t s) {
     if (use_r1()) return gs_launch_render_backward_r1(va, recs, point_list, ranges, n_contrib, final_T, dL_dcolor, dL_ddepth, dL_dalpha, sg, s);
     dim3 grid(va.tiles_x, va.tiles_y);
-    // ring depth, queued visits per flush, partial blocks, CTAs per SM: 2 x 6 KB ring + 2 x 20 KB partial blocks + 34 KB
-    // queue = 92 KB, two CTAs per SM.  Measured on an H100 SXM against 8 visits per flush (75 KB, three CTAs per SM; the
-    // moments' fp32 summation order then changes too), a third ring stage, and a third partial block with the refill
-    // issued before the combine: all slower.
-    constexpr int ST = 2, SL = 16, PB = 2, MB = 2;
-    constexpr size_t smem = bwd_smem_bytes(ST, SL, PB);
-    static const cudaError_t attr = cudaFuncSetAttribute(composite_backward_kernel<ST, SL, PB, MB>,
-                                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    GS_CUDA_CHECK(attr);
-    composite_backward_kernel<ST, SL, PB, MB><<<grid, NTHREADS, smem, s>>>(va, recs, point_list, ranges, n_contrib, final_T,
-                                                                          dL_dcolor, dL_ddepth, dL_dalpha, sg);
+    GS_CUDA_CHECK(bwd_kernel_attributes());
+    BWD_KERNEL<<<grid, NTHREADS, BWD_SMEM, s>>>(va, recs, point_list, ranges, n_contrib, final_T, dL_dcolor, dL_ddepth,
+                                                dL_dalpha, sg);
     gs_count_launches(1);
     GS_CUDA_CHECK(cudaGetLastError());
+    return 0;
+}
+
+extern "C" int32_t gs_b200_composite_bwd_occupancy(int32_t* ctas_per_sm, int32_t* smem_bytes) {
+    if (!ctas_per_sm || !smem_bytes) { gs_set_error("composite_bwd_occupancy: NULL"); return 1; }
+    GS_CUDA_CHECK(bwd_kernel_attributes());
+    int n = 0;
+    GS_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, BWD_KERNEL, NTHREADS, BWD_SMEM));
+    *ctas_per_sm = n;
+    *smem_bytes = (int32_t)BWD_SMEM;
     return 0;
 }

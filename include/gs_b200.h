@@ -98,6 +98,11 @@ int32_t gs_b200_get_tile_culling(void);
  * Initial value from the environment variable GS_B200_COMPOSITE ("r1" selects 1). */
 int32_t gs_b200_debug_set_composite(int32_t mode);
 
+/* Measurement query (no reference counterpart): CTAs per SM of the round-2 composite backward kernel as the CUDA
+ * occupancy calculator reports it for the current device, with the kernel's launch attributes applied, and the
+ * kernel's dynamic shared memory per CTA in bytes. */
+int32_t gs_b200_composite_bwd_occupancy(int32_t* ctas_per_sm, int32_t* smem_bytes);
+
 /* Forward — replaces `_C.rasterize_gaussians` as called from
  * GaussianRasterizer.forward (main_3DGS_renderer.py:927-936).
  *   M        number of SH coefficients per channel in `shs` ([N,M,3]); ignored when colors_precomp != NULL
