@@ -202,15 +202,102 @@ int32_t gs_b200_sort_pairs_u32(uint32_t* keys, uint32_t* keys_alt, uint32_t* val
     return rc;
 }
 
-// ---- forward, split at the one host round-trip (number of (tile,splat) pairs) -----------------
-// Phase A: preprocess -> depth sort -> gather-scan -> async D2H of the pair count.
-// Phase B (needs P on the host to size the binning buffers): emit -> tile sort -> ranges -> composite.
+// ---- binning of nv views ----------------------------------------------------------------------------------
+// Inputs are the preprocess's [nv][N] arrays (one view: the single-view entries; a chunk of views: the multi-view
+// step).  Every stage is one launch (or one launch per digit pass) over all nv views.
+// Phase A: segmented depth sort -> segmented gather-scan -> ONE D2H of the nv pair totals.
+// Phase B (the host has the totals, to size the pair buffers): emit (which also counts the tile sort's digit
+// histograms) -> segmented tile sort -> ranges.  View v's pairs are [base[v], base[v+1]) of one chunk buffer.
+struct BinA {
+    int nv = 0, N = 0, dbg = 0;
+    uint32_t *tiles = nullptr, *dkeys = nullptr, *ids = nullptr;          // [nv][N] from the preprocess
+    const uint32_t* minkeys = nullptr; int minkey_stride = 0;             // depth-key bias of view v: minkeys[v * stride]
+    uint32_t *dkeys_alt = nullptr, *ids_alt = nullptr, *offsets = nullptr;
+    unsigned long long* totals = nullptr;                                 // [nv] on the device
+    void *sort_scratch = nullptr, *scan_scratch = nullptr;
+    const uint32_t* sorted_ids = nullptr;                                 // [nv][N], set by bin_a
+};
+static size_t bin_a_bytes(int nv, int N) {
+    const size_t nn = (size_t)nv * N;
+    return Carver::need(nn, 4) * 3 + Carver::need(nv, 8) + Carver::need(gs_sort_seg_scratch_bytes(nv, (int64_t)nn), 1) +
+           Carver::need(gs_scan_seg_scratch_bytes(N, nv), 1);
+}
+static void carve_bin_a(Carver& c, BinA& b, int nv, int N) {
+    const size_t nn = (size_t)nv * N;
+    b.nv = nv; b.N = N;
+    b.dkeys_alt = c.take<uint32_t>(nn); b.ids_alt = c.take<uint32_t>(nn); b.offsets = c.take<uint32_t>(nn);
+    b.totals = c.take<unsigned long long>(nv);
+    b.sort_scratch = c.take<char>(gs_sort_seg_scratch_bytes(nv, (int64_t)nn));
+    b.scan_scratch = c.take<char>(gs_scan_seg_scratch_bytes(N, nv));
+}
+static int bin_a(BinA& b, unsigned long long* host_totals, cudaStream_t s) {
+    SortSegs sg; sg.n = b.nv;
+    for (int v = 0; v <= b.nv; v++) sg.off[v] = (int64_t)v * b.N;
+    int in_alt = 0;
+    { StageTimer t(1, s);
+    if (gs_sort_pairs_segmented(b.dkeys, b.dkeys_alt, b.ids, b.ids_alt, sg, 0, 32, b.sort_scratch, &in_alt, b.minkeys,
+                                b.minkey_stride, false, s)) return 1; }
+    STAGE_CHECK(b.dbg, s, "depth sort");
+    b.sorted_ids = in_alt ? b.ids_alt : b.ids;
+    { StageTimer t(2, s);
+    if (gs_scan_gather_seg_u32(b.tiles, b.sorted_ids, b.offsets, b.totals, b.N, b.nv, b.scan_scratch, s)) return 1; }
+    GS_CUDA_CHECK(cudaMemcpyAsync(host_totals, b.totals, (size_t)b.nv * 8, cudaMemcpyDeviceToHost, s));
+    return 0;
+}
+// per-view pair bases from the totals phase A copied to the host
+static int view_spans(int nv, const unsigned long long* host_totals, ViewSpans& vs) {
+    vs.n = nv; vs.base[0] = 0;
+    for (int v = 0; v < nv; v++) {
+        if (host_totals[v] >= (1ull << 30)) { gs_set_error("too many (tile,splat) pairs in one view: %llu", host_totals[v]); return 1; }
+        vs.base[v + 1] = vs.base[v] + (int64_t)host_totals[v];
+    }
+    return 0;
+}
+struct BinB { uint32_t *point_list = nullptr, *tile_keys = nullptr, *keys_alt = nullptr, *vals_alt = nullptr; void* sort_scratch = nullptr; };
+static size_t bin_b_scratch_bytes(int nv, int64_t P) {
+    return Carver::need(P, 4) * 2 + Carver::need(gs_sort_seg_scratch_bytes(nv, P), 1);
+}
+static void carve_bin_b_scratch(Carver& c, BinB& o, int nv, int64_t P) {
+    o.keys_alt = c.take<uint32_t>(P); o.vals_alt = c.take<uint32_t>(P);
+    o.sort_scratch = c.take<char>(gs_sort_seg_scratch_bytes(nv, P));
+}
+// ranges: [nv][tiles][2], zeroed by the caller
+static int bin_b(const BinA& a, const ViewSpans& vs, int tiles_x, int tiles_y, const SplatRec* recs, const uint4* spans,
+          const BinB& o, uint32_t* ranges, cudaStream_t s) {
+    const int64_t P = vs.base[vs.n];
+    if (P <= 0) return 0;
+    const int ntiles = tiles_x * tiles_y;
+    const int tbits = bits_for(ntiles);
+    const int npasses = (tbits + 7) / 8;
+    // start in the buffer that makes the last pass land in the saved pair
+    uint32_t *k0 = (npasses & 1) ? o.keys_alt : o.tile_keys, *v0 = (npasses & 1) ? o.vals_alt : o.point_list;
+    uint32_t *k1 = (npasses & 1) ? o.tile_keys : o.keys_alt, *v1 = (npasses & 1) ? o.point_list : o.vals_alt;
+    GS_CUDA_CHECK(cudaMemsetAsync(o.sort_scratch, 0, gs_sort_hist_bytes(vs.n), s));
+    { StageTimer t(3, s);
+    if (gs_launch_emit_multi(recs, spans, a.sorted_ids, a.offsets, a.N, tiles_x, tiles_y, vs, k0, v0,
+                             (uint32_t*)o.sort_scratch, npasses, s)) return 1; }
+    STAGE_CHECK(a.dbg, s, "emit");
+    SortSegs sg; sg.n = vs.n;
+    for (int v = 0; v <= vs.n; v++) sg.off[v] = vs.base[v];
+    int in_alt = 0;
+    { StageTimer t(4, s);
+    if (gs_sort_pairs_segmented(k0, k1, v0, v1, sg, 0, tbits, o.sort_scratch, &in_alt, nullptr, 0, true, s)) return 1; }
+    STAGE_CHECK(a.dbg, s, "tile sort");
+    { StageTimer t(5, s);
+    if (gs_launch_ranges_multi(o.tile_keys, vs, ntiles, ranges, s)) return 1; }
+    STAGE_CHECK(a.dbg, s, "ranges");
+    return 0;
+}
+
+// ---- single-view forward, split at the one host round-trip (number of (tile,splat) pairs) -----------------
+// Phase A: preprocess -> binning phase A (one view) -> async D2H of the pair count.
+// Phase B (needs P on the host to size the binning buffers): binning phase B -> composite.
 struct FwdCtx {
     ViewArgs va; int N = 0, M = 0, dbg = 0;
     Allocator A;
     gs_b200_state* state = nullptr;
     SplatRec* recs = nullptr;
-    uint32_t *sorted_ids = nullptr, *offsets = nullptr;
+    BinA bin;
     uint4* spans = nullptr;                        // tile culling: per-row tile spans (NULL = full squares)
     unsigned long long* host_total = nullptr;      // pinned
     float *out_color = nullptr, *out_depth = nullptr, *out_alpha = nullptr;
@@ -218,14 +305,10 @@ struct FwdCtx {
     FwdCtx(gs_b200_alloc_fn fn, void* user, cudaStream_t st) : A{fn, user, st}, s(st) {}
 };
 
-// per-view arrays already produced by the multi-view preprocess (gs_launch_preprocess_multi)
-struct PreView { SplatRec* recs; uint32_t *tiles, *dkeys, *ids, *min_key; uint4* spans; };
-
 static int fwd_phase_a(FwdCtx& c, const gs_b200_view* view, int32_t N, int32_t M, const float* means3D,
                        const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
                        const float* rotations, const float* cov3D_precomp, float* out_color, float* out_depth,
-                       float* out_alpha, int32_t* radii, gs_b200_state* state, unsigned long long* host_total,
-                       const PreView* pre = nullptr) {
+                       float* out_alpha, int32_t* radii, gs_b200_state* state, unsigned long long* host_total) {
     cudaStream_t s = c.s;
     if (make_view_args(view, c.va)) return 1;
     if (check_inputs(N, M, view->sh_degree, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp)) return 1;
@@ -248,48 +331,30 @@ static int fwd_phase_a(FwdCtx& c, const gs_b200_view* view, int32_t N, int32_t M
     state->final_T = ci.take<float>(npix);
     GS_CUDA_CHECK(cudaMemsetAsync(state->ranges, 0, (size_t)ntiles * 2 * 4, s));
 
-    if (pre) c.recs = pre->recs;
-    else c.recs = (SplatRec*)A.get(GS_B200_BUF_GEOM, (size_t)N * sizeof(SplatRec), &state->owned[GS_B200_BUF_GEOM]);
+    c.recs = (SplatRec*)A.get(GS_B200_BUF_GEOM, (size_t)N * sizeof(SplatRec), &state->owned[GS_B200_BUF_GEOM]);
     if (A.failed) return 1;
     state->geom = c.recs;
     *host_total = 0;
     if (N > 0) {
-        const size_t sort_b = gs_sort_scratch_bytes(N), scan_b = gs_scan_scratch_bytes(N);
-        const bool own_spans = !pre && g_tile_culling.load() == 2;
-        const size_t sc_bytes = Carver::need(N, 4) * 6 + Carver::need(1, 8) * 2 + Carver::need(sort_b, 1) + Carver::need(scan_b, 1) +
-                                (own_spans ? Carver::need(N, 16) : 0);
+        const bool own_spans = g_tile_culling.load() == 2;
+        const size_t sc_bytes = Carver::need(N, 4) * 3 + Carver::need(1, 8) + bin_a_bytes(1, N) + (own_spans ? Carver::need(N, 16) : 0);
         void* sc = A.get(GS_B200_BUF_SCRATCH, sc_bytes);
         if (A.failed) return 1;
         Carver cv(sc);
-        c.spans = pre ? pre->spans : (own_spans ? cv.take<uint4>(N) : nullptr);
-        uint32_t* tiles = cv.take<uint32_t>(N);
-        uint32_t* dkeys = cv.take<uint32_t>(N);
-        uint32_t* ids = cv.take<uint32_t>(N);
-        if (pre) { tiles = pre->tiles; dkeys = pre->dkeys; ids = pre->ids; }
-        uint32_t* dkeys_alt = cv.take<uint32_t>(N);
-        uint32_t* ids_alt = cv.take<uint32_t>(N);
-        c.offsets = cv.take<uint32_t>(N);
-        unsigned long long* total = cv.take<unsigned long long>(1);
+        c.spans = own_spans ? cv.take<uint4>(N) : nullptr;
+        BinA& b = c.bin;
+        b.tiles = cv.take<uint32_t>(N);
+        b.dkeys = cv.take<uint32_t>(N);
+        b.ids = cv.take<uint32_t>(N);
         uint32_t* min_key = (uint32_t*)cv.take<unsigned long long>(1);
-        void* sort_scratch = cv.take<char>(sort_b);
-        void* scan_scratch = cv.take<char>(scan_b);
-        if (pre) {
-            min_key = pre->min_key;       // the multi-view pass has already written records, keys, tiles, spans and radii
-        } else {
-            GS_CUDA_CHECK(cudaMemsetAsync(min_key, 0xFF, 4, s));
-            StageTimer t(0, s);
-            if (gs_launch_preprocess(va, N, M, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
-                                     c.recs, radii, tiles, dkeys, ids, min_key, c.spans, s)) return 1;
-        }
+        carve_bin_a(cv, b, 1, N);
+        b.minkeys = min_key; b.dbg = c.dbg;
+        GS_CUDA_CHECK(cudaMemsetAsync(min_key, 0xFF, 4, s));
+        { StageTimer t(0, s);
+        if (gs_launch_preprocess(va, N, M, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
+                                 c.recs, radii, b.tiles, b.dkeys, b.ids, min_key, c.spans, s)) return 1; }
         STAGE_CHECK(c.dbg, s, "preprocess");
-        int in_alt = 0;
-        { StageTimer t(1, s);
-        if (gs_sort_pairs_u32_biased(dkeys, dkeys_alt, ids, ids_alt, N, 0, 32, sort_scratch, &in_alt, min_key, s)) return 1; }
-        STAGE_CHECK(c.dbg, s, "depth sort");
-        c.sorted_ids = in_alt ? ids_alt : ids;
-        { StageTimer t(2, s);
-        if (gs_scan_gather_u32(tiles, c.sorted_ids, c.offsets, total, N, scan_scratch, s)) return 1; }
-        GS_CUDA_CHECK(cudaMemcpyAsync(host_total, total, 8, cudaMemcpyDeviceToHost, s));
+        if (bin_a(b, host_total, s)) return 1;
     }
     return 0;
 }
@@ -300,39 +365,23 @@ static int fwd_phase_b_bin(FwdCtx& c) {
     const ViewArgs& va = c.va;
     gs_b200_state* state = c.state;
     Allocator& A = c.A;
-    const unsigned long long P = *c.host_total;
-    const int ntiles = va.tiles_x * va.tiles_y;
-    if (P >= (1ull << 30)) { gs_set_error("too many (tile,splat) pairs: %llu", P); return 1; }
-    state->num_rendered = (int64_t)P;
+    ViewSpans vs;
+    if (view_spans(1, c.host_total, vs)) return 1;
+    const int64_t P = vs.base[1];
+    state->num_rendered = P;
     const size_t bin_bytes = Carver::need(P, 4) * 2;
     void* bin = A.get(GS_B200_BUF_BINNING, bin_bytes, &state->owned[GS_B200_BUF_BINNING]);
     if (A.failed) return 1;
     Carver cb(bin);
-    state->point_list = cb.take<uint32_t>(P);
-    state->tile_keys = cb.take<uint32_t>(P);
+    BinB o;
+    o.point_list = state->point_list = cb.take<uint32_t>(P);
+    o.tile_keys = state->tile_keys = cb.take<uint32_t>(P);
     if (P > 0) {
-        const size_t sort_b = gs_sort_scratch_bytes((int64_t)P);
-        void* sc2 = A.get(GS_B200_BUF_SCRATCH, Carver::need(P, 4) * 2 + Carver::need(sort_b, 1));
+        void* sc2 = A.get(GS_B200_BUF_SCRATCH, bin_b_scratch_bytes(1, P));
         if (A.failed) return 1;
         Carver c2(sc2);
-        uint32_t* keys_b = c2.take<uint32_t>(P);
-        uint32_t* vals_b = c2.take<uint32_t>(P);
-        void* sort_scratch = c2.take<char>(sort_b);
-        const int tbits = bits_for(ntiles);
-        const int npasses = (tbits + 7) / 8;
-        // start in the buffer that makes the last pass land in the saved pair
-        uint32_t *k0 = (npasses & 1) ? keys_b : state->tile_keys, *v0 = (npasses & 1) ? vals_b : state->point_list;
-        uint32_t *k1 = (npasses & 1) ? state->tile_keys : keys_b, *v1 = (npasses & 1) ? state->point_list : vals_b;
-        { StageTimer t(3, s);
-        if (gs_launch_emit(c.recs, c.spans, c.sorted_ids, c.offsets, c.N, va.tiles_x, va.tiles_y, k0, v0, s)) return 1; }
-        STAGE_CHECK(c.dbg, s, "emit");
-        int in_alt = 0;
-        { StageTimer t(4, s);
-        if (gs_sort_pairs_u32(k0, k1, v0, v1, (int64_t)P, 0, tbits, sort_scratch, &in_alt, s)) return 1; }
-        STAGE_CHECK(c.dbg, s, "tile sort");
-        { StageTimer t(5, s);
-        if (gs_launch_ranges(state->tile_keys, (int64_t)P, state->ranges, s)) return 1; }
-        STAGE_CHECK(c.dbg, s, "ranges");
+        carve_bin_b_scratch(c2, o, 1, P);
+        if (bin_b(c.bin, vs, va.tiles_x, va.tiles_y, c.recs, c.spans, o, state->ranges, s)) return 1;
     }
     return 0;
 }
@@ -422,24 +471,18 @@ int32_t gs_b200_knn_mean_dist2(const float* points, int32_t N, float* out, void*
 // ---------------------------------------------------------------------------------
 // Multi-view optimisation step (device-resident or host buffers).
 //
-// Views are software-pipelined over TWO internal streams with per-slot grow-only
-// workspaces (no allocation in steady state): while view v's composite kernels
-// (instruction-issue bound) run on one stream, view v+1's preprocess / sorts
-// (memory bound) run on the other, and the host's wait for v+1's pair count is
-// hidden behind the GPU work already queued for v.
+// Views are handled in chunks.  An auxiliary stream projects and bins every view of a chunk in batched launches
+// (one host wait for the chunk's pair counts); the views' composite kernels then run on TWO slot streams with
+// per-slot grow-only workspaces (no allocation in steady state), so that one view's forward overlaps the other's
+// backward.
 // ---------------------------------------------------------------------------------
 namespace {
 
 struct Region { void* p = nullptr; size_t cap = 0; };
 struct Slot {
     cudaStream_t stream = nullptr;
-    Region saved[3];                 // GEOM, BINNING, IMAGE
-    Region arena; size_t arena_off = 0, arena_want = 0;
-    std::vector<void*> overflow;
-    Region sgrad, radii, image, loss_ws;
-    unsigned long long* host_total = nullptr;
-    cudaEvent_t evA = nullptr, evDone = nullptr;
-    bool failed = false;
+    Region image, loss_ws, nc;       // nc: n_contrib + final_T of the view on the slot
+    cudaEvent_t evDone = nullptr;
 
     static int ensure(Region& r, size_t bytes, cudaStream_t st) {
         if (r.cap >= bytes) return 0;
@@ -449,61 +492,41 @@ struct Slot {
         r.cap = want;
         return 0;
     }
-    void begin_call() {
-        // grow the arena to what the previous call needed in total (so overflow is a warm-up-only path)
-        if (arena_want > arena.cap) { release_overflow(); ensure(arena, arena_want, stream); }
-        arena_off = 0; arena_want = 0;
-    }
-    void release_overflow() {
-        if (overflow.empty()) return;
-        cudaStreamSynchronize(stream);
-        for (void* p : overflow) cudaFree(p);
-        overflow.clear();
-    }
-    void* alloc(int tag, size_t bytes) {
-        bytes = (bytes + 255) & ~(size_t)255;
-        if (tag != GS_B200_BUF_SCRATCH) {
-            if (ensure(saved[tag], bytes, stream)) { failed = true; return nullptr; }
-            return saved[tag].p;
-        }
-        arena_want += bytes;
-        if (arena_off + bytes <= arena.cap) { void* p = (char*)arena.p + arena_off; arena_off += bytes; return p; }
-        void* p = nullptr;
-        if (cudaMalloc(&p, bytes) != cudaSuccess) { failed = true; gs_set_error("cudaMalloc(%zu) failed", bytes); return nullptr; }
-        overflow.push_back(p);
-        return p;
-    }
 };
-void* slot_alloc_cb(void* user, int32_t tag, size_t bytes) { return ((Slot*)user)->alloc(tag, bytes); }
 
-constexpr int NSLOTS = 8;       // the device-resident step alternates between slots 0 and 1; the host-buffer step bins up to 8 views ahead
+constexpr int NSLOTS = 2;       // the composites of a chunk's views alternate between two slot streams
 struct StepCache {
     Slot slot[NSLOTS];
     bool init = false;
     cudaStream_t copy_stream = nullptr, d2h_stream = nullptr, aux_stream = nullptr;
-    cudaEvent_t evFork = nullptr, evPB = nullptr, evGeom = nullptr, evColour = nullptr, evD2H = nullptr, evAux = nullptr, evPre[2] = {nullptr, nullptr};
+    cudaEvent_t evFork = nullptr, evPB = nullptr, evGeom = nullptr, evD2H = nullptr, evAux = nullptr;
+    cudaEvent_t evBinA[2] = {nullptr, nullptr}, evBin[2] = {nullptr, nullptr};
+    unsigned long long* host_totals[2] = {nullptr, nullptr};     // pinned: per-view pair counts of a chunk
     std::vector<cudaEvent_t> up_ready;          // per view: upstream gradient resident
     Region host_stage;                           // device copies of host inputs (step_host)
     bool busy = false;                           // a view hook must not re-enter the step entries on this thread
-    Region ws_recs[2], ws_sg[2], ws_u32[2], ws_spans[2];               // per-chunk [VB][N] arrays of the multi-view step
+    // per-chunk workspaces of the multi-view step, two sets that alternate between chunks: [VB][N] arrays of the
+    // preprocess and the depth sort, the binning scratch and ranges, and the chunk's pair lists
+    Region ws_recs[2], ws_sg[2], ws_u32[2], ws_spans[2], ws_bin[2], ws_pairs[2];
     int ensure_init() {
         if (init) return 0;
         for (int i = 0; i < NSLOTS; i++) {
             GS_CUDA_CHECK(cudaStreamCreateWithFlags(&slot[i].stream, cudaStreamNonBlocking));
-            GS_CUDA_CHECK(cudaEventCreateWithFlags(&slot[i].evA, cudaEventDisableTiming));
             GS_CUDA_CHECK(cudaEventCreateWithFlags(&slot[i].evDone, cudaEventDisableTiming));
-            GS_CUDA_CHECK(cudaHostAlloc((void**)&slot[i].host_total, 64, cudaHostAllocDefault));
         }
         GS_CUDA_CHECK(cudaStreamCreateWithFlags(&copy_stream, cudaStreamNonBlocking));
         GS_CUDA_CHECK(cudaStreamCreateWithFlags(&d2h_stream, cudaStreamNonBlocking));
         GS_CUDA_CHECK(cudaStreamCreateWithFlags(&aux_stream, cudaStreamNonBlocking));
         GS_CUDA_CHECK(cudaEventCreateWithFlags(&evAux, cudaEventDisableTiming));
-        for (int i = 0; i < 2; i++) GS_CUDA_CHECK(cudaEventCreateWithFlags(&evPre[i], cudaEventDisableTiming));
+        for (int i = 0; i < 2; i++) {
+            GS_CUDA_CHECK(cudaEventCreateWithFlags(&evBinA[i], cudaEventDisableTiming));
+            GS_CUDA_CHECK(cudaEventCreateWithFlags(&evBin[i], cudaEventDisableTiming));
+            GS_CUDA_CHECK(cudaHostAlloc((void**)&host_totals[i], GS_MAX_SEGS * sizeof(unsigned long long), cudaHostAllocDefault));
+        }
         GS_CUDA_CHECK(cudaEventCreateWithFlags(&evD2H, cudaEventDisableTiming));
         GS_CUDA_CHECK(cudaEventCreateWithFlags(&evFork, cudaEventDisableTiming));
         GS_CUDA_CHECK(cudaEventCreateWithFlags(&evPB, cudaEventDisableTiming));
         GS_CUDA_CHECK(cudaEventCreateWithFlags(&evGeom, cudaEventDisableTiming));
-        GS_CUDA_CHECK(cudaEventCreateWithFlags(&evColour, cudaEventDisableTiming));
         init = true;
         return 0;
     }
@@ -530,9 +553,10 @@ PackedPtrs carve_packed(float* base, size_t N, size_t M, bool with_m2d) {
 }
 
 // Device-resident core.  views_host gives tanfov per view (host side), views_dev the matrices.
-// Views are handled in chunks of <= VB: ONE multi-view preprocess pass over the Gaussians for the chunk
-// (parameters read once), then per view [depth sort -> scan -> (host: pair count) -> emit -> tile sort ->
-// ranges -> composite fwd -> composite bwd] pipelined over the two slot streams, then ONE multi-view
+// Views are handled in chunks of <= VB.  Per chunk, on the aux stream: ONE multi-view preprocess pass over the
+// Gaussians (parameters read once), then the batched binning of all its views (segmented depth sort, gather-scan,
+// one host wait for the pair counts, emit, segmented tile sort, ranges).  Then per view, on the slot streams:
+// composite forward -> view hook -> SplatGrad zeroing -> composite backward.  Then ONE multi-view
 // preprocess-backward pass (parameters read once, gradients written once).
 // grad_sink (optional): called after each Gaussian range [first, first+count) of the FINAL preprocess-backward has
 // been enqueued on `user`, so a host-buffer caller can start the D2H of that range while the next one computes.
@@ -541,9 +565,8 @@ struct GradSink { void (*fn)(void* ctx, int first, int count, cudaStream_t user)
 // its backward is; the callee enqueues, on that stream, whatever turns images[v] into dL_dout[v] (the loss).
 // forward_only: no backward at all (render entry).  radii_out (optional): [V][N] per-view radii.
 // shs_ready (optional, host-buffer step): the SH block is still being uploaded when the step starts -- `user` is ordered
-// after the geometry parameters only.  Projection, depth sort and binning of every view run first (colour-free), the
-// colours are filled in when the event fires, then the composites follow.  Needs one slot per view: V <= NSLOTS, else
-// the step simply waits for the event first.
+// after the geometry parameters only.  Projection and binning of each chunk run first (colour-free), the colours are
+// filled in when the event fires (sh_colour_multi on the aux stream), then the composites follow.
 struct StepOpts { gs_b200_view_hook hook = nullptr; void* hook_user = nullptr; bool forward_only = false; int32_t* radii_out = nullptr;
                   cudaEvent_t shs_ready = nullptr; };
 
@@ -568,142 +591,147 @@ int step_core(int V, int H, int W, int sh_degree, float scale_modifier, const fl
         sink = &user_sink;
     }
     const size_t npix = (size_t)H * W;
-    // View chunks: one batched preprocess / preprocess-backward pass per chunk of <= 16 views, on the aux stream:
-    //   aux stream:   pre(0) | pre(1) ............ bwd(0) | pre(2) ....... bwd(1) | ... | bwd(last)
-    //   slot streams:          views of chunk 0 ........... views of chunk 1 ......
-    // pre(k+1) is enqueued when chunk k's views start, bwd(k) when they have all been enqueued; two workspace sets
-    // alternate and the aux stream's own order (bwd(k-1) before pre(k+1)) protects their reuse.
+    const int tiles_x = (W + GS_TILE - 1) / GS_TILE, tiles_y = (H + GS_TILE - 1) / GS_TILE, ntiles = tiles_x * tiles_y;
+    // View chunks: one batched preprocess + binning / preprocess-backward per chunk of <= 16 views, on the aux stream:
+    //   aux stream:   pre+bin(0) | pre+bin(1) ......... bwd(0) | pre+bin(2) ...... bwd(1) | ... | bwd(last)
+    //   slot streams:             views of chunk 0 ............. views of chunk 1 .......
+    // pre+bin(k+1) is enqueued when chunk k's views start (its second half, after the host has read the pair counts,
+    // once they have all been enqueued), bwd(k) after that; two workspace sets alternate and the aux stream's own
+    // order (bwd(k-1) before pre(k+1)) protects their reuse.
     // GS_B200_STEP_OVERLAP=1 additionally cuts a step of >= 6 views into two chunks so that the batched passes overlap
-    // the composites instead of running alone at the head and tail of the step.  Measured on C1 (8 views): 12.25-12.33
-    // ms vs 12.09-12.10 ms without — every kernel of the step is issue-bound, so the overlapped passes only take
-    // issue slots from the composites, and the second chunk re-reads the parameters.  Off by default.
-    const int maxv = std::min(gs_preprocess_multi_max_views(), 16);
+    // the composites instead of running alone at the head and tail of the step.  Measured on C1 (8 views, B200,
+    // before the binning was batched): 12.25-12.33 ms vs 12.09-12.10 ms without — every kernel of the step is
+    // issue-bound, so the overlapped passes only take issue slots from the composites, and the second chunk re-reads
+    // the parameters.  Off by default.
+    const int maxv = std::min(gs_preprocess_multi_max_views(), GS_MAX_SEGS);
     static const bool overlap = []() { const char* e = getenv("GS_B200_STEP_OVERLAP"); return e && e[0] == '1'; }();
     const int nchunks = std::max((overlap && V >= 6) ? 2 : 1, (V + maxv - 1) / maxv);
     const int VB = (V + nchunks - 1) / nchunks;
     const size_t nvb = (size_t)VB * N;
     const bool tight = g_tile_culling.load() >= 1;
-    const bool late = O.shs_ready && nchunks == 1 && V <= NSLOTS && par.shs && !par.colors;
+    const bool late = O.shs_ready && par.shs && !par.colors;
     if (O.shs_ready && !late) GS_CUDA_CHECK(cudaStreamWaitEvent(user, O.shs_ready, 0));
-    const int nslots_used = late ? V : 2;
-    auto slot_of = [&](int j) { return late ? j : (j & 1); };
-    struct WS { SplatRec* recs; SplatGrad* sg; int32_t* radii; uint32_t *tiles, *dkeys, *ids, *minkeys; uint4* spans; } ws[2];
+    struct WS { SplatRec* recs; SplatGrad* sg; int32_t* radii; uint32_t *minkeys, *ranges; uint4* spans; BinA bin; } ws[2];
     const int nsets = nchunks > 1 ? 2 : 1;
+    const size_t ranges_bytes = Carver::need((size_t)VB * ntiles * 2, 4);
     for (int i = 0; i < nsets; i++) {
         if (Slot::ensure(C.ws_recs[i], nvb * sizeof(SplatRec), user) || Slot::ensure(C.ws_sg[i], nvb * sizeof(SplatGrad), user) ||
-            Slot::ensure(C.ws_u32[i], nvb * 4 * 4 + 256 * 4, user)) return 1;
+            Slot::ensure(C.ws_u32[i], nvb * 4 * 4 + 256 * 4, user) ||
+            Slot::ensure(C.ws_bin[i], bin_a_bytes(VB, N) + ranges_bytes, user)) return 1;
         if (tight && Slot::ensure(C.ws_spans[i], nvb * sizeof(uint4), user)) return 1;
         uint32_t* u32 = (uint32_t*)C.ws_u32[i].p;
-        ws[i] = WS{(SplatRec*)C.ws_recs[i].p, (SplatGrad*)C.ws_sg[i].p, (int32_t*)u32, u32 + nvb, u32 + 2 * nvb, u32 + 3 * nvb,
-                   u32 + 4 * nvb /* [VB] stride 2 words */, tight ? (uint4*)C.ws_spans[i].p : nullptr};
+        WS& w = ws[i];
+        w.recs = (SplatRec*)C.ws_recs[i].p; w.sg = (SplatGrad*)C.ws_sg[i].p; w.radii = (int32_t*)u32;
+        w.minkeys = u32 + 4 * nvb;        // [VB] stride 2 words
+        w.spans = tight ? (uint4*)C.ws_spans[i].p : nullptr;
+        w.bin.tiles = u32 + nvb; w.bin.dkeys = u32 + 2 * nvb; w.bin.ids = u32 + 3 * nvb;
+        w.bin.minkeys = w.minkeys; w.bin.minkey_stride = 2;
+        Carver cb(C.ws_bin[i].p);
+        w.ranges = cb.take<uint32_t>((size_t)VB * ntiles * 2);
+        carve_bin_a(cb, w.bin, VB, N);
     }
     cudaStream_t aux = C.aux_stream;
     // everything is ordered after the caller's stream
     GS_CUDA_CHECK(cudaEventRecord(C.evFork, user));
     GS_CUDA_CHECK(cudaStreamWaitEvent(aux, C.evFork, 0));
 
-    auto enqueue_pre = [&](int k) -> int {           // batched preprocess of chunk k on the aux stream
+    int64_t rendered = 0;
+    ViewSpans vsp[2];
+    BinB pairs[2];
+    // first half of chunk k's projection and binning on the aux stream: preprocess, depth sort, scan, pair counts D2H
+    auto enqueue_pre = [&](int k) -> int {
         const int v0 = k * VB, nv = std::min(VB, V - v0);
-        const WS& w = ws[k & (nsets - 1)];
+        WS& w = ws[k & (nsets - 1)];
         GS_CUDA_CHECK(cudaMemsetAsync(w.minkeys, 0xFF, 256 * 4, aux));
         { StageTimer t(0, aux);
         if (gs_launch_preprocess_multi(views_dev + (size_t)v0 * 40, nv, W, H, sh_degree, scale_modifier, N, M, par.means,
-                                       par.shs, par.colors, par.opac, par.scales, par.rots, w.recs, w.radii, w.tiles, w.dkeys, w.ids,
-                                       w.minkeys, w.spans, aux, late ? 1 : 0)) return 1; }
-        GS_CUDA_CHECK(cudaEventRecord(C.evPre[k & 1], aux));
+                                       par.shs, par.colors, par.opac, par.scales, par.rots, w.recs, w.radii, w.bin.tiles,
+                                       w.bin.dkeys, w.bin.ids, w.minkeys, w.spans, aux, late ? 1 : 0)) return 1; }
+        w.bin.nv = nv;
+        if (bin_a(w.bin, C.host_totals[k & 1], aux)) return 1;
+        GS_CUDA_CHECK(cudaEventRecord(C.evBinA[k & 1], aux));
+        return 0;
+    };
+    // second half, once the chunk's pair counts are on the host: pair buffers, emit, tile sort, ranges (+ colours)
+    auto enqueue_bin = [&](int k) -> int {
+        const int v0 = k * VB, nv = std::min(VB, V - v0);
+        const int q = k & (nsets - 1);
+        WS& w = ws[q];
+        GS_CUDA_CHECK(cudaEventSynchronize(C.evBinA[k & 1]));
+        ViewSpans& vs = vsp[k & 1];
+        if (view_spans(nv, C.host_totals[k & 1], vs)) return 1;
+        const int64_t P = vs.base[nv];
+        rendered += P;
+        // grow-only: the pair lists of all the chunk's views live until its last composite backward
+        if (Slot::ensure(C.ws_pairs[q], Carver::need(P, 4) * 2 + bin_b_scratch_bytes(nv, P), aux)) return 1;
+        Carver cp(C.ws_pairs[q].p);
+        BinB& o = pairs[k & 1];
+        o.point_list = cp.take<uint32_t>(P); o.tile_keys = cp.take<uint32_t>(P);
+        carve_bin_b_scratch(cp, o, nv, P);
+        GS_CUDA_CHECK(cudaMemsetAsync(w.ranges, 0, (size_t)nv * ntiles * 2 * 4, aux));
+        if (bin_b(w.bin, vs, tiles_x, tiles_y, w.recs, w.spans, o, w.ranges, aux)) return 1;
+        if (late) {
+            GS_CUDA_CHECK(cudaStreamWaitEvent(aux, O.shs_ready, 0));
+            if (gs_launch_sh_colour_multi(views_dev + (size_t)v0 * 40, nv, sh_degree, N, M, par.means, par.shs, w.radii, w.recs, aux)) return 1;
+        }
+        GS_CUDA_CHECK(cudaEventRecord(C.evBin[k & 1], aux));
         return 0;
     };
 
-    gs_b200_state st[NSLOTS];
-    gs_b200_view view[NSLOTS];
-    std::unique_ptr<FwdCtx> ctx[NSLOTS];            // released on every exit path
-    int64_t rendered = 0;
     int rc = enqueue_pre(0);
-
+    if (!rc) rc = enqueue_bin(0);
     for (int k = 0; k < nchunks && !rc; k++) {
         const int v0 = k * VB, nv = std::min(VB, V - v0);
         const WS& w = ws[k & (nsets - 1)];
-        // the slot streams continue after this chunk's preprocess ...
-        for (int i = 0; i < nslots_used; i++) GS_CUDA_CHECK(cudaStreamWaitEvent(C.slot[i].stream, C.evPre[k & 1], 0));
-        // ... while the next chunk's preprocess already runs beside them
+        const ViewSpans& vs = vsp[k & 1];
+        const BinB& o = pairs[k & 1];
+        // the slot streams continue after this chunk's binning ...
+        for (int i = 0; i < NSLOTS; i++) GS_CUDA_CHECK(cudaStreamWaitEvent(C.slot[i].stream, C.evBin[k & 1], 0));
+        // ... while the next chunk's preprocess and depth sort already run beside them
         if (k + 1 < nchunks && (rc = enqueue_pre(k + 1))) break;
 
-        auto launch_a = [&](int j) -> int {          // j: view index inside the chunk
-            const int q = slot_of(j);
-            Slot& S = C.slot[q];
-            S.begin_call();
-            if (!images_dev && Slot::ensure(S.image, 5 * npix * 4, S.stream)) return 1;
+        for (int j = 0; j < nv && !rc; j++) {
+            Slot& S = C.slot[j & 1];
             const int v = v0 + j;
+            if (!images_dev && Slot::ensure(S.image, 5 * npix * 4, S.stream)) { rc = 1; break; }
+            if (Slot::ensure(S.nc, Carver::need(npix, 4) * 2, S.stream)) { rc = 1; break; }
             const float* vh = views_host + (size_t)v * 40;
             const float* vd = views_dev + (size_t)v * 40;
-            gs_b200_view& vw = view[q];
+            gs_b200_view vw;
             vw.image_height = H; vw.image_width = W; vw.tanfovx = vh[38]; vw.tanfovy = vh[39];
             vw.bg = vd + 35; vw.scale_modifier = scale_modifier; vw.viewmatrix = vd; vw.projmatrix = vd + 16;
             vw.sh_degree = sh_degree; vw.campos = vd + 32; vw.prefiltered = 0; vw.debug = 0;
+            ViewArgs va;
+            if ((rc = make_view_args(&vw, va))) break;
             float* img = images_dev ? images_dev + (size_t)v * 5 * npix : (float*)S.image.p;
-            ctx[q].reset(new FwdCtx(slot_alloc_cb, &S, S.stream));
-            const size_t o = (size_t)j * N;
-            PreView pre{w.recs + o, w.tiles + o, w.dkeys + o, w.ids + o, w.minkeys + 2 * j, w.spans ? w.spans + o : nullptr};
-            if (fwd_phase_a(*ctx[q], &vw, N, M, par.means, par.shs, par.colors, par.opac, par.scales, par.rots, nullptr,
-                            img, img + 3 * npix, img + 4 * npix, w.radii + o, &st[q], S.host_total, &pre)) return 1;
-            GS_CUDA_CHECK(cudaEventRecord(S.evA, S.stream));
-            // The view's SplatGrad slice is zeroed here, on its slot stream, so the write overlaps the other slot's
-            // composites instead of delaying the batched preprocess.  Also for a view without pairs, whose composite
-            // backward is skipped: the batched preprocess-backward reads the slice for every Gaussian with radii > 0.
-            // (Placed after evA, so the host's wait for the pair count does not wait for it too.)
-            if (!O.forward_only) GS_CUDA_CHECK(cudaMemsetAsync(w.sg + o, 0, (size_t)N * sizeof(SplatGrad), S.stream));
-            return S.failed ? 1 : 0;
-        };
-
-        // after view j's forward has been enqueued: loss hook, upstream-gradient wait, composite backward
-        auto finish_view = [&](int j) -> int {
-            const int q = slot_of(j);
-            Slot& S = C.slot[q];
-            const int v = v0 + j;
-            if (O.forward_only) return S.failed ? 1 : 0;
-            if (O.hook && O.hook(O.hook_user, v, (void*)S.stream) != 0) { gs_set_error("step: view hook failed at view %d", v); return 1; }
+            Carver cn(S.nc.p);
+            uint32_t* n_contrib = cn.take<uint32_t>(npix);
+            float* final_T = cn.take<float>(npix);
+            const size_t off = (size_t)j * N;
+            const SplatRec* recs = w.recs + off;
+            const uint32_t* point_list = o.point_list + vs.base[j];
+            const uint32_t* ranges = w.ranges + (size_t)j * ntiles * 2;
+            { StageTimer t(6, S.stream);
+            if ((rc = gs_launch_render_forward(va, recs, point_list, ranges, img, img + 3 * npix, img + 4 * npix,
+                                               n_contrib, final_T, S.stream))) break; }
+            if (O.forward_only) continue;
+            if (O.hook && O.hook(O.hook_user, v, (void*)S.stream) != 0) { gs_set_error("step: view hook failed at view %d", v); rc = 1; break; }
             const float* up = dL_dout_dev + (size_t)v * 5 * npix;
             if (up_ready) GS_CUDA_CHECK(cudaStreamWaitEvent(S.stream, up_ready[v], 0));
-            if (st[q].num_rendered > 0) {
+            // The view's SplatGrad slice is zeroed here, on its slot stream, so the write overlaps the other slot's
+            // composites.  Also for a view without pairs, whose composite backward is skipped: the batched
+            // preprocess-backward reads the slice for every Gaussian with radii > 0.
+            GS_CUDA_CHECK(cudaMemsetAsync(w.sg + off, 0, (size_t)N * sizeof(SplatGrad), S.stream));
+            if (vs.base[j + 1] > vs.base[j]) {
                 StageTimer t(7, S.stream);
-                if (gs_launch_render_backward(ctx[q]->va, (const SplatRec*)st[q].geom, st[q].point_list, st[q].ranges, st[q].n_contrib,
-                                              st[q].final_T, up, up + 3 * npix, up + 4 * npix, w.sg + (size_t)j * N, S.stream)) return 1;
-            }
-            return S.failed ? 1 : 0;
-        };
-        if (late) {
-            // every view's depth sort and binning first (one slot per view, no colour needed) ...
-            for (int j = 0; j < nv && !rc; j++) rc = launch_a(j);
-            for (int j = 0; j < nv && !rc; j++) {
-                GS_CUDA_CHECK(cudaEventSynchronize(C.slot[j].evA));
-                if ((rc = fwd_phase_b_bin(*ctx[j]))) break;
-                rendered += st[j].num_rendered;
-            }
-            // ... the colours as soon as the SH block has arrived, then the composites
-            if (!rc) {
-                GS_CUDA_CHECK(cudaStreamWaitEvent(aux, O.shs_ready, 0));
-                rc = gs_launch_sh_colour_multi(views_dev + (size_t)v0 * 40, nv, sh_degree, N, M, par.means, par.shs, w.radii, w.recs, aux);
-                if (!rc) GS_CUDA_CHECK(cudaEventRecord(C.evColour, aux));
-            }
-            for (int j = 0; j < nv && !rc; j++) {
-                GS_CUDA_CHECK(cudaStreamWaitEvent(C.slot[j].stream, C.evColour, 0));
-                if ((rc = fwd_phase_b_render(*ctx[j]))) break;
-                rc = finish_view(j);
-            }
-        } else {
-            rc = launch_a(0);
-            for (int j = 0; j < nv && !rc; j++) {
-                Slot& S = C.slot[j & 1];
-                if (j + 1 < nv) { rc = launch_a(j + 1); if (rc) break; }
-                GS_CUDA_CHECK(cudaEventSynchronize(S.evA));
-                if ((rc = fwd_phase_b(*ctx[j & 1]))) break;
-                rendered += st[j & 1].num_rendered;
-                rc = finish_view(j);
+                if ((rc = gs_launch_render_backward(va, recs, point_list, ranges, n_contrib, final_T, up, up + 3 * npix,
+                                                    up + 4 * npix, w.sg + off, S.stream))) break;
             }
         }
-        for (int i = 0; i < NSLOTS; i++) ctx[i].reset();
+        // the next chunk's binning, now that this chunk's views are queued behind it
+        if (!rc && k + 1 < nchunks) rc = enqueue_bin(k + 1);
         // the aux stream picks up after this chunk's views (batched backward, radii copy, workspace hand-over)
-        for (int i = 0; i < nslots_used; i++) {
+        for (int i = 0; i < NSLOTS; i++) {
             cudaEventRecord(C.slot[i].evDone, C.slot[i].stream);
             cudaStreamWaitEvent(aux, C.slot[i].evDone, 0);
         }
@@ -724,7 +752,7 @@ int step_core(int V, int H, int W, int sh_degree, float scale_modifier, const fl
         }
     }
     // join: the caller's stream continues after the aux stream (which has waited for both slot streams)
-    for (int i = 0; i < nslots_used; i++) {          // (on an error path the slots may not have been joined into aux yet)
+    for (int i = 0; i < NSLOTS; i++) {          // (on an error path the slots may not have been joined into aux yet)
         cudaEventRecord(C.slot[i].evDone, C.slot[i].stream);
         cudaStreamWaitEvent(aux, C.slot[i].evDone, 0);
     }

@@ -183,22 +183,40 @@ int gs_launch_activate(int, const float*, const float*, const float*, float*, fl
 int gs_launch_adam(int, int, const float*, float, float, float, int, float, const float*, float*, float*, float*, cudaStream_t);
 int gs_launch_densify_stats(int, const float*, const int32_t*, float*, float*, float*, cudaStream_t);
 
+// Segmented sort (gs_sort.cu): n segments [off[i], off[i+1]) of one key array, sorted independently in one
+// launch per digit pass.  The multi-view step sorts the depth keys and the tile keys of all views of a chunk so.
+constexpr int GS_MAX_SEGS = 16;
+struct SortSegs { int n; int64_t off[GS_MAX_SEGS + 1]; };
+
 size_t gs_sort_scratch_bytes(int64_t n);
+size_t gs_sort_seg_scratch_bytes(int nseg, int64_t total_n);
+size_t gs_sort_hist_bytes(int nseg);       // head of the scratch: digit histograms [segment][4][256] u32
 int gs_sort_pairs_u32(uint32_t* keys, uint32_t* keys_alt, uint32_t* vals, uint32_t* vals_alt, int64_t n,
                       int begin_bit, int end_bit, void* scratch, int* result_in_alt, cudaStream_t s);
-
-int gs_sort_pairs_u32_biased(uint32_t* keys, uint32_t* keys_alt, uint32_t* vals, uint32_t* vals_alt, int64_t n,
-                             int begin_bit, int end_bit, void* scratch, int* result_in_alt,
-                             const uint32_t* key_bias, cudaStream_t s);
+// key_bias (may be NULL): subtracted from segment i's keys is key_bias[i * bias_stride].  hist_ready: the caller has
+// zeroed the histogram head of the scratch and counted every segment's digits into it (see gs_launch_emit_multi).
+int gs_sort_pairs_segmented(uint32_t* keys, uint32_t* keys_alt, uint32_t* vals, uint32_t* vals_alt, const SortSegs& segs,
+                            int begin_bit, int end_bit, void* scratch, int* result_in_alt, const uint32_t* key_bias,
+                            int bias_stride, bool hist_ready, cudaStream_t s);
 
 size_t gs_scan_scratch_bytes(int64_t n);
+size_t gs_scan_seg_scratch_bytes(int64_t n, int nseg);
 // offsets[i] = exclusive prefix of tiles[ids[i]] (ids may be NULL -> identity); total[0] = sum.
 int gs_scan_gather_u32(const uint32_t* tiles, const uint32_t* ids, uint32_t* offsets, unsigned long long* total,
                        int64_t n, void* scratch, cudaStream_t s);
+// the same over nseg segments of n elements back to back (ids index inside their segment); totals[nseg]
+int gs_scan_gather_seg_u32(const uint32_t* tiles, const uint32_t* ids, uint32_t* offsets, unsigned long long* totals,
+                           int64_t n, int nseg, void* scratch, cudaStream_t s);
 
-int gs_launch_emit(const SplatRec* recs, const uint4* spans, const uint32_t* sorted_ids, const uint32_t* offsets, int N,
-                   int tiles_x, int tiles_y, uint32_t* tile_keys, uint32_t* vals, cudaStream_t s);
-int gs_launch_ranges(const uint32_t* sorted_tile_keys, int64_t P, uint32_t* ranges, cudaStream_t s);
+// Binning of nv views (gs_binning.cu).  Inputs are [nv][N] arrays; view v's pairs go to [base[v], base[v] + P[v]) of
+// one chunk buffer.  The emit also counts the digit histograms of the tile sort into hist ([view][4][256], zeroed).
+struct ViewSpans { int n; int64_t base[GS_MAX_SEGS + 1]; };      // base[n] = total pairs
+int gs_launch_emit_multi(const SplatRec* recs, const uint4* spans, const uint32_t* sorted_ids, const uint32_t* offsets,
+                         int N, int tiles_x, int tiles_y, const ViewSpans& vs, uint32_t* tile_keys, uint32_t* vals,
+                         uint32_t* hist, int hist_passes, cudaStream_t s);
+// ranges [nv][tiles][2] of the tile-sorted chunk buffer (zeroed by the caller)
+int gs_launch_ranges_multi(const uint32_t* sorted_tile_keys, const ViewSpans& vs, int ntiles, uint32_t* ranges,
+                           cudaStream_t s);
 
 int gs_launch_render_forward(const ViewArgs& va, const SplatRec* recs, const uint32_t* point_list,
                              const uint32_t* ranges, float* out_color, float* out_depth, float* out_alpha,
