@@ -2,9 +2,9 @@
 #include "../../include/ngp_b200.h"
 #include "gs_common.cuh"
 
-int ngp_grid_encode_fwd(const float*, long long, const float*, const int32_t*, int, float, float, int, float*, cudaStream_t);
-int ngp_grid_encode_bwd(const float*, long long, const int32_t*, int, float, float, int, const float*, float*, cudaStream_t);
-int ngp_grid_tv(const float*, long long, const float*, const int32_t*, int, float, float, int, float, float*, cudaStream_t);
+int ngp_grid_encode_fwd(const float*, long long, const float*, const int32_t*, int, float, double, int, float*, cudaStream_t);
+int ngp_grid_encode_bwd(const float*, long long, const int32_t*, int, float, double, int, const float*, float*, cudaStream_t);
+int ngp_grid_tv(const float*, long long, const float*, const int32_t*, int, float, double, int, float, float*, cudaStream_t);
 size_t ngp_march_scratch_bytes(long long, int);
 int ngp_march_count(const float*, const float*, long long, const uint8_t*, int, const float*, float, float, float, const float*,
                     uint32_t*, uint32_t*, unsigned long long*, void*, cudaStream_t);
@@ -25,18 +25,18 @@ int ngp_mlp2_bwd(const float*, long long, int, int, int, const float*, const flo
 
 extern "C" {
 int32_t ngp_b200_grid_encode_fwd(const float* x, int64_t N, const float* emb, const int32_t* offsets, int32_t L, float bound,
-                                 float pls, int32_t base, float* out, void* stream) {
+                                 double pls, int32_t base, float* out, void* stream) {
     NGP_REQ(N == 0 || (x && emb && offsets && out), "NULL pointer");
     NGP_REQ(((size_t)emb & 7) == 0 && ((size_t)out & 7) == 0, "emb/out must be 8-byte aligned");
     return ngp_grid_encode_fwd(x, N, emb, offsets, L, bound, pls, base, out, (cudaStream_t)stream);
 }
-int32_t ngp_b200_grid_encode_bwd(const float* x, int64_t N, const int32_t* offsets, int32_t L, float bound, float pls,
+int32_t ngp_b200_grid_encode_bwd(const float* x, int64_t N, const int32_t* offsets, int32_t L, float bound, double pls,
                                  int32_t base, const float* g, float* d_emb, void* stream) {
     NGP_REQ(N == 0 || (x && offsets && g && d_emb), "NULL pointer");
     return ngp_grid_encode_bwd(x, N, offsets, L, bound, pls, base, g, d_emb, (cudaStream_t)stream);
 }
 int32_t ngp_b200_grid_tv_grad(const float* x, int64_t N, const float* emb, const int32_t* offsets, int32_t L, float bound,
-                              float pls, int32_t base, float weight, float* d_emb, void* stream) {
+                              double pls, int32_t base, float weight, float* d_emb, void* stream) {
     NGP_REQ(N == 0 || (x && emb && offsets && d_emb), "NULL pointer");
     return ngp_grid_tv(x, N, emb, offsets, L, bound, pls, base, weight, d_emb, (cudaStream_t)stream);
 }

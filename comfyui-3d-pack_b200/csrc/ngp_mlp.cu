@@ -148,18 +148,28 @@ mlp2_bwd_kernel(const float* __restrict__ X, long long N, const float* __restric
             }
         }
         __syncthreads();
-        // weight gradients over the tile: thread t owns outputs [t*PER, t*PER+PER) of the flattened [H][DIN] matrix
+        // weight gradients over the tile: thread t owns outputs [t*PER, t*PER+PER) of the flattened [H][DIN] matrix.
+        // The tile's 128 samples are summed on their own and the tile sum is added to the CTA's total: a CTA of the
+        // persistent grid sees ~N / 396 samples (50 k at 2e7 rows), and one running fp32 sum over all of them drifts
+        // ~sqrt(50 k) u from the exact gradient, several times torch's fp32 GEMM
         {
             const int first = threadIdx.x * PER;
             const int k = first / DIN, j0 = first - k * DIN;
+            float t1[PER];
+#pragma unroll
+            for (int i = 0; i < PER; i++) t1[i] = 0.f;
             for (int s = 0; s < MT; s++) {
                 const float g = sGH[s * (H + 1) + k];
 #pragma unroll
-                for (int i = 0; i < PER; i++) acc1[i] = fmaf(g, sX[s * (DIN + 1) + j0 + i], acc1[i]);
+                for (int i = 0; i < PER; i++) t1[i] = fmaf(g, sX[s * (DIN + 1) + j0 + i], t1[i]);
             }
+#pragma unroll
+            for (int i = 0; i < PER; i++) acc1[i] += t1[i];
             if (threadIdx.x < DOUT * H) {
                 const int o = threadIdx.x / H, kk = threadIdx.x - o * H;
-                for (int s = 0; s < MT; s++) acc2 = fmaf(sGY[s * 4 + o], sA[s * (H + 1) + kk], acc2);
+                float t2 = 0.f;
+                for (int s = 0; s < MT; s++) t2 = fmaf(sGY[s * 4 + o], sA[s * (H + 1) + kk], t2);
+                acc2 += t2;
             }
         }
         __syncthreads();
@@ -183,8 +193,15 @@ template <int DIN, int H, int DOUT>
 int launch_bwd(const float* X, long long N, const float* W1, const float* W2, const float* GY, float* GX, float* GW1,
                float* GW2, cudaStream_t s) {
     const size_t smem = (size_t)(2 * DIN * H + 4 * H + MT * (DIN + 1) + 2 * MT * (H + 1) + MT * 4) * 4;
-    static bool set = false;
-    if (!set) { cudaFuncSetAttribute(mlp2_bwd_kernel<DIN, H, DOUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); set = true; }
+    // the attribute belongs to the (device, kernel) pair: set it once per device the process launches on
+    static unsigned long long set_mask = 0;
+    int devi = 0;
+    GS_CUDA_CHECK(cudaGetDevice(&devi));
+    const unsigned long long bit = devi < 64 ? 1ull << devi : 0ull;
+    if (!(set_mask & bit)) {
+        GS_CUDA_CHECK(cudaFuncSetAttribute(mlp2_bwd_kernel<DIN, H, DOUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        set_mask |= bit;
+    }
     const long long tiles_ = (N + MT - 1) / MT; const int grid = (int)(tiles_ < GS_NUM_SMS * 3 ? tiles_ : GS_NUM_SMS * 3);
     mlp2_bwd_kernel<DIN, H, DOUT><<<grid, MT, smem, s>>>(X, N, W1, W2, GY, GX, GW1, GW2);
     return 0;
@@ -192,10 +209,10 @@ int launch_bwd(const float* X, long long N, const float* W1, const float* W2, co
 
 #define MLP_DISPATCH(FN, ...)                                                              \
     do {                                                                                   \
-        if (Din == 24) { switch (Dout) { case 1: FN<24, 32, 1>(__VA_ARGS__); break; case 2: FN<24, 32, 2>(__VA_ARGS__); break; \
-                                         case 3: FN<24, 32, 3>(__VA_ARGS__); break; default: FN<24, 32, 4>(__VA_ARGS__); } }  \
-        else { switch (Dout) { case 1: FN<32, 32, 1>(__VA_ARGS__); break; case 2: FN<32, 32, 2>(__VA_ARGS__); break;           \
-                               case 3: FN<32, 32, 3>(__VA_ARGS__); break; default: FN<32, 32, 4>(__VA_ARGS__); } }            \
+        if (Din == 24) { switch (Dout) { case 1: rc = FN<24, 32, 1>(__VA_ARGS__); break; case 2: rc = FN<24, 32, 2>(__VA_ARGS__); break; \
+                                         case 3: rc = FN<24, 32, 3>(__VA_ARGS__); break; default: rc = FN<24, 32, 4>(__VA_ARGS__); } }  \
+        else { switch (Dout) { case 1: rc = FN<32, 32, 1>(__VA_ARGS__); break; case 2: rc = FN<32, 32, 2>(__VA_ARGS__); break;           \
+                               case 3: rc = FN<32, 32, 3>(__VA_ARGS__); break; default: rc = FN<32, 32, 4>(__VA_ARGS__); } }            \
     } while (0)
 
 }  // namespace
@@ -207,7 +224,9 @@ int ngp_mlp2_supported(int Din, int H, int Dout) {
 int ngp_mlp2_fwd(const float* X, long long N, int Din, int H, int Dout, const float* W1, const float* W2, float* Y, cudaStream_t s) {
     if (N <= 0) return 0;
     if (!ngp_mlp2_supported(Din, H, Dout)) { gs_set_error("mlp2: unsupported dims %d-%d-%d", Din, H, Dout); return 1; }
+    int rc = 0;
     MLP_DISPATCH(launch_fwd, X, N, W1, W2, Y, s);
+    if (rc) return rc;
     gs_count_launches(1);
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
@@ -217,7 +236,9 @@ int ngp_mlp2_bwd(const float* X, long long N, int Din, int H, int Dout, const fl
                  float* GX, float* GW1, float* GW2, cudaStream_t s) {
     if (N <= 0) return 0;
     if (!ngp_mlp2_supported(Din, H, Dout)) { gs_set_error("mlp2: unsupported dims %d-%d-%d", Din, H, Dout); return 1; }
+    int rc = 0;
     MLP_DISPATCH(launch_bwd, X, N, W1, W2, GY, GX, GW1, GW2, s);
+    if (rc) return rc;
     gs_count_launches(1);
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;

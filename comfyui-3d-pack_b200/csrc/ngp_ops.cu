@@ -274,7 +274,9 @@ weights_fwd_kernel(const float* __restrict__ ts, const float* __restrict__ te, c
     const int s = ranges[2 * r], c = ranges[2 * r + 1];
     float T = 1.f;
     for (int i = s; i < s + c; i++) {
-        const float a = 1.f - __expf(-sig[i] * (te[i] - ts[i]));
+        // -expm1f: alpha to ~1 ulp of itself.  1 - __expf(-x) cancels for the small sigma * dt of empty space (a 2-ulp
+        // error of exp near 1 is ~1e-7 absolute, all of alpha at x = 1e-7) and would also trail nerfacc's 1 - exp(-x)
+        const float a = -expm1f(-sig[i] * (te[i] - ts[i]));
         w[i] = T * a; tr[i] = T; al[i] = a;
         T *= 1.f - a;
     }
@@ -325,10 +327,13 @@ accumulate_bwd_kernel(const float* __restrict__ w, const float* __restrict__ v, 
     dw[i] = g;
 }
 
-int make_meta(GridMeta& gm, const int32_t* offsets_host, int L, float bound, float pls, int base) {
+int make_meta(GridMeta& gm, const int32_t* offsets_host, int L, float bound, double pls, int base) {
     if (L <= 0 || L > NGP_MAX_LEVELS) { gs_set_error("grid: num_levels must be 1..%d", NGP_MAX_LEVELS); return 1; }
     gm.L = L; gm.bound = bound;
-    const float S = log2f(pls);
+    // torch-ngp's S: log2 in double, then rounded to fp32.  log2f of the fp32-rounded scale is one ulp above it for
+    // 2^(1/3) (config 3), which turns the integer scales 31, 63, 127, ... into 31.000004, ... and every third
+    // resolution into res + 1 (levels 3 and 6 then overflow their dense tables and get hashed)
+    const float S = (float)log2(pls);
     for (int l = 0; l < L; l++) {
         gm.scale[l] = exp2f((float)l * S) * (float)base - 1.0f;
         gm.res[l] = (int)ceilf(gm.scale[l]) + 1;
@@ -343,7 +348,7 @@ int make_meta(GridMeta& gm, const int32_t* offsets_host, int L, float bound, flo
 #define NGP_GRID(n) (unsigned)(((n) + 255) / 256), 256
 
 int ngp_grid_encode_fwd(const float* x, long long N, const float* emb, const int32_t* offsets_host, int L, float bound,
-                        float pls, int base, float* out, cudaStream_t s) {
+                        double pls, int base, float* out, cudaStream_t s) {
     if (N <= 0) return 0;
     GridMeta gm; if (make_meta(gm, offsets_host, L, bound, pls, base)) return 1;
     grid_encode_fwd_kernel<<<NGP_GRID(N * L), 0, s>>>(x, N, (const float2*)emb, gm, (float2*)out);
@@ -351,7 +356,7 @@ int ngp_grid_encode_fwd(const float* x, long long N, const float* emb, const int
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
 }
-int ngp_grid_encode_bwd(const float* x, long long N, const int32_t* offsets_host, int L, float bound, float pls, int base,
+int ngp_grid_encode_bwd(const float* x, long long N, const int32_t* offsets_host, int L, float bound, double pls, int base,
                         const float* g_out, float* d_emb, cudaStream_t s) {
     if (N <= 0) return 0;
     GridMeta gm; if (make_meta(gm, offsets_host, L, bound, pls, base)) return 1;
@@ -375,7 +380,7 @@ int ngp_grid_encode_bwd(const float* x, long long N, const int32_t* offsets_host
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
 }
-int ngp_grid_tv(const float* x, long long N, const float* emb, const int32_t* offsets_host, int L, float bound, float pls,
+int ngp_grid_tv(const float* x, long long N, const float* emb, const int32_t* offsets_host, int L, float bound, double pls,
                 int base, float weight, float* d_emb, cudaStream_t s) {
     if (N <= 0) return 0;
     GridMeta gm; if (make_meta(gm, offsets_host, L, bound, pls, base)) return 1;

@@ -112,12 +112,13 @@ DR_EXPORTS = ["dr_b200_rasterize_scratch_bytes", "dr_b200_rasterize_fwd", "dr_b2
 # ---- Instant-NGP path (include/ngp_b200.h) -----------------------------------------------------------------
 _L = C.c_int64
 _F = C.c_float
+_D = C.c_double
 lib.ngp_b200_grid_encode_fwd.restype = _I
-lib.ngp_b200_grid_encode_fwd.argtypes = [_P, _L, _P, _P, _I, _F, _F, _I, _P, _P]
+lib.ngp_b200_grid_encode_fwd.argtypes = [_P, _L, _P, _P, _I, _F, _D, _I, _P, _P]
 lib.ngp_b200_grid_encode_bwd.restype = _I
-lib.ngp_b200_grid_encode_bwd.argtypes = [_P, _L, _P, _I, _F, _F, _I, _P, _P, _P]
+lib.ngp_b200_grid_encode_bwd.argtypes = [_P, _L, _P, _I, _F, _D, _I, _P, _P, _P]
 lib.ngp_b200_grid_tv_grad.restype = _I
-lib.ngp_b200_grid_tv_grad.argtypes = [_P, _L, _P, _P, _I, _F, _F, _I, _F, _P, _P]
+lib.ngp_b200_grid_tv_grad.argtypes = [_P, _L, _P, _P, _I, _F, _D, _I, _F, _P, _P]
 lib.ngp_b200_march_scratch_bytes.restype = C.c_size_t
 lib.ngp_b200_march_scratch_bytes.argtypes = [_L, _I]
 lib.ngp_b200_march_count.restype = _I

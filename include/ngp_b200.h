@@ -18,17 +18,19 @@ extern "C" {
 
 /* ---- hash grid (level_dim C = 2) ------------------------------------------------------------------
  * x[N,3] in [-bound,bound]; emb[offsets[L], 2]; offsets = HOST array of L+1 int32 (entries per level, computed
- * as the package does); out[N, 2L].  per-level scale = 2^(l*log2(per_level_scale))*base_res - 1, resolution = ceil(scale)+1;
+ * as the package does); out[N, 2L].  per-level scale = 2^(l*S)*base_res - 1 in fp32 with S = (float)log2(per_level_scale)
+ * taken in double (as torch-ngp does: the scale of config 3's levels 3, 6, 9, ... is an integer only that way),
+ * resolution = ceil(scale)+1;
  * dense indexing while (res+1)^3 <= level size, else XOR hash with primes {1, 2654435761, 805459861}. */
 int32_t ngp_b200_grid_encode_fwd(const float* x, int64_t N, const float* emb, const int32_t* offsets, int32_t L,
-                                 float bound, float per_level_scale, int32_t base_resolution, float* out, void* stream);
+                                 float bound, double per_level_scale, int32_t base_resolution, float* out, void* stream);
 /* d_emb is ADDED to (caller zeroes) */
 int32_t ngp_b200_grid_encode_bwd(const float* x, int64_t N, const int32_t* offsets, int32_t L, float bound,
-                                 float per_level_scale, int32_t base_resolution, const float* dL_dout, float* d_emb,
+                                 double per_level_scale, int32_t base_resolution, const float* dL_dout, float* d_emb,
                                  void* stream);
 /* GridEncoder.grad_total_variation: adds weight * L1-TV gradient at the cells containing x[N,3] to d_emb */
 int32_t ngp_b200_grid_tv_grad(const float* x, int64_t N, const float* emb, const int32_t* offsets, int32_t L,
-                              float bound, float per_level_scale, int32_t base_resolution, float weight, float* d_emb,
+                              float bound, double per_level_scale, int32_t base_resolution, float weight, float* d_emb,
                               void* stream);
 
 /* ---- occupancy-grid marching ---------------------------------------------------------------------------

@@ -168,8 +168,9 @@ def march(rays_o, rays_d, binary: torch.Tensor, aabb: torch.Tensor, near, far, d
         t_enter = t_enter + t_offset
     hit = t_exit > t_enter
     dtf = torch.tensor(dt, dtype=f32)
-    kmax = int(math.ceil(float(((t_exit - t_enter).clamp_min(0)).max()) / dt)) + 1 if n else 0
-    k = torch.arange(kmax, dtype=f32)[None, :]
+    span = torch.where(hit, t_exit - t_enter, torch.zeros_like(t_exit))     # NaN for rays in a face plane (no hit)
+    kmax = int(math.ceil(float(span.max()) / dt)) + 1 if n else 0
+    k = torch.arange(kmax, dtype=f32, device=rays_o.device)[None, :]     # (runs on CUDA tensors too: same fp32 ops)
     ts = t_enter[:, None] + k * dtf
     te = t_enter[:, None] + (k + 1.0) * dtf
     tm = (ts + te) * 0.5
