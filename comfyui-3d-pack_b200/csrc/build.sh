@@ -10,7 +10,7 @@ pids=()
 # preprocess forward: NO FMA contraction (bit-exact integer outputs vs the oracle)
 $NVCC $COMMON -fmad=false -c gs_preprocess.cu -o build/gs_preprocess.o & pids+=($!)
 $NVCC $COMMON -fmad=false -c dr_raster.cu -o build/dr_raster.o & pids+=($!)
-for f in gs_sort gs_binning gs_render gs_composite gs_backward gs_knn gs_train gs_densify gs_loss gs_capi dr_ops dr_capi ngp_ops ngp_mlp ngp_capi ngp_mcubes; do
+for f in gs_sort gs_binning gs_composite gs_backward gs_knn gs_train gs_densify gs_loss gs_capi dr_ops dr_capi ngp_ops ngp_mlp ngp_capi ngp_mcubes; do
   $NVCC $COMMON -c $f.cu -o build/$f.o & pids+=($!)
 done
 for p in "${pids[@]}"; do wait $p; done

@@ -598,14 +598,8 @@ int step_core(int V, int H, int W, int sh_degree, float scale_modifier, const fl
     // pre+bin(k+1) is enqueued when chunk k's views start (its second half, after the host has read the pair counts,
     // once they have all been enqueued), bwd(k) after that; two workspace sets alternate and the aux stream's own
     // order (bwd(k-1) before pre(k+1)) protects their reuse.
-    // GS_B200_STEP_OVERLAP=1 additionally cuts a step of >= 6 views into two chunks so that the batched passes overlap
-    // the composites instead of running alone at the head and tail of the step.  Measured on C1 (8 views, B200,
-    // before the binning was batched): 12.25-12.33 ms vs 12.09-12.10 ms without — every kernel of the step is
-    // issue-bound, so the overlapped passes only take issue slots from the composites, and the second chunk re-reads
-    // the parameters.  Off by default.
     const int maxv = std::min(gs_preprocess_multi_max_views(), GS_MAX_SEGS);
-    static const bool overlap = []() { const char* e = getenv("GS_B200_STEP_OVERLAP"); return e && e[0] == '1'; }();
-    const int nchunks = std::max((overlap && V >= 6) ? 2 : 1, (V + maxv - 1) / maxv);
+    const int nchunks = (V + maxv - 1) / maxv;
     const int VB = (V + nchunks - 1) / nchunks;
     const size_t nvb = (size_t)VB * N;
     const bool tight = g_tile_culling.load() >= 1;
@@ -791,7 +785,7 @@ int step_host_impl(int32_t V, int32_t H, int32_t W, int32_t sh_degree, float sca
     // H2D order on the copy stream: geometry parameters FIRST (projection, sorting and binning need nothing else), then
     // the SH block (192 of the 236 B per Gaussian at degree 3; only the colours and the backward need it -- step_core
     // bins every view while it is on its way, StepOpts::shs_ready), then the upstream gradients view by view (needed only
-    // at each view's backward), so they stream in behind the compute.  GS_B200_HOST_LATE_SH=0: wait for everything first.
+    // at each view's backward), so they stream in behind the compute.
     GS_CUDA_CHECK(cudaEventRecord(C.evFork, s));
     GS_CUDA_CHECK(cudaStreamWaitEvent(C.copy_stream, C.evFork, 0));
     GS_CUDA_CHECK(cudaMemcpyAsync(d_views, views_host, (size_t)V * 160, cudaMemcpyHostToDevice, C.copy_stream));
@@ -807,10 +801,9 @@ int step_host_impl(int32_t V, int32_t H, int32_t W, int32_t sh_degree, float sca
                                       cudaMemcpyHostToDevice, C.copy_stream));
         GS_CUDA_CHECK(cudaEventRecord(C.up_ready[v], C.copy_stream));
     }
-    static const bool late_sh = []() { const char* e = getenv("GS_B200_HOST_LATE_SH"); return !(e && e[0] == '0'); }();
-    GS_CUDA_CHECK(cudaStreamWaitEvent(s, late_sh ? C.evGeom : C.evPB, 0));
+    GS_CUDA_CHECK(cudaStreamWaitEvent(s, C.evGeom, 0));
     StepOpts opts;
-    if (late_sh) opts.shs_ready = C.evPB;
+    opts.shs_ready = C.evPB;
     // D2H of the summed gradients is chunked over Gaussian ranges and starts as soon as a range is final
     struct SinkCtx { StepCache* C; float* host; float* dev; size_t N, M; } sctx{&C, grads_host, d_grad, (size_t)N, (size_t)M};
     GradSink sink;

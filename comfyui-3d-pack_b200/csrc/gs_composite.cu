@@ -14,9 +14,8 @@
 //    the 8x8 quadrant (w&1, w>>1); every lane owns TWO pixels (x, y) and (x, y+4),
 //    so dx and every per-splat operand are loaded and set up once for two
 //    pixels (the pixel pair is carried as one 64-bit register pair);
-//  * the tile's records are gathered by three 16 B cp.async per record (or, in the
-//    forward with GS_B200_GATHER=tma, one 48 B cp.async.bulk) into a ring of shared-memory
-//    stages, each completed on an mbarrier; a warp releases a stage with one
+//  * the tile's records are gathered by three 16 B cp.async per record into a ring of
+//    shared-memory stages, each completed on an mbarrier; a warp releases a stage with one
 //    shared-memory atomic and the last of the four to release it refills it.
 //    There is no __syncthreads() in the main loops;
 //  * each warp decides by itself which records of a stage can reach
@@ -35,7 +34,6 @@
 //    of each splat in fp64, in fixed warp order, and ONE fp64 red.global.add per value and
 //    (tile, splat) leaves the CTA (SplatGrad in gs_common.cuh says why fp64).
 #include "gs_common.cuh"
-#include <stdlib.h>
 
 namespace {
 
@@ -83,16 +81,13 @@ __device__ __forceinline__ float ex2_approx(float x) { float y; asm("ex2.approx.
 __device__ __forceinline__ float rcp_approx(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float lg2_approx(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
-// ---- mbarrier / bulk-copy helpers ---------------------------------------------------------------
+// ---- mbarrier helpers ---------------------------------------------------------------------------
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
 }
 __device__ __forceinline__ void mbar_fence_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
     asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n\t}" ::"r"(bar), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     asm volatile(
@@ -102,11 +97,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         "@p bra D_%=;\n\t"
         "bra W_%=;\n\t"
         "D_%=:\n\t}" ::"r"(bar), "r"(parity), "r"(1000000u) : "memory");   // suspend-time hint (ns): sleep in hardware, do not poll
-}
-// one record: global -> shared through the bulk-copy engine, completion counted on `bar`
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
 __device__ __forceinline__ float lds32(uint32_t addr) {
     float v;
@@ -205,13 +195,13 @@ struct RingState {
     __device__ __forceinline__ void advance(int nstages) { if (++stage == (uint32_t)nstages) { stage = 0; phase ^= 1u; } }
 };
 
-// gather of one stage: ids (coalesced LDG), then per record either three 16 B cp.async (LDGSTS) per lane with one
-// cp.async.mbarrier.arrive.noinc per lane (the stage's mbarrier expects 32 arrivals) -- the default -- or
-// (GS_B200_GATHER=tma) ONE 48 B bulk copy through the TMA engine (UBLKCP; completion = bytes counted on the stage's
-// mbarrier, which one expect_tx arrival arms).  UBLKCP takes its operands from uniform registers, so a per-lane
-// gather serialises into a ~9-instruction loop per record inside the issuing warp, whereas the three LDGSTS are one
-// warp-wide instruction each.
-template <bool KEEP_IDS, bool TMA>
+// gather of one stage: ids (coalesced LDG), then three 16 B cp.async (LDGSTS) per record and lane, and one
+// cp.async.mbarrier.arrive.noinc per lane, so the stage's mbarrier expects STAGE_ARRIVALS = 32 arrivals.  (One 48 B
+// bulk copy per record through the TMA engine would be fewer copies, but UBLKCP takes its operands from uniform
+// registers, so a per-lane gather serialises into a ~9-instruction loop per record inside the issuing warp, whereas the
+// three LDGSTS are one warp-wide instruction each.)
+constexpr uint32_t STAGE_ARRIVALS = 32;
+template <bool KEEP_IDS>
 __device__ __forceinline__ void produce_stage(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ list, int n,
                                               uint32_t s_rec, uint32_t s_ids, uint32_t bar, int lane) {
     uint32_t id[BATCH / 32];
@@ -228,31 +218,20 @@ __device__ __forceinline__ void produce_stage(const SplatRec* __restrict__ recs,
         }
         __syncwarp();
     }
-    if (TMA) {
-        if (lane == 0) mbar_arrive_expect_tx(bar, (uint32_t)n * REC_BYTES);
-        __syncwarp();
 #pragma unroll
-        for (int i = 0; i < BATCH / 32; i++) {
-            const int j = i * 32 + lane;
-            if (j < n) bulk_g2s(s_rec + j * REC_BYTES, recs + id[i], REC_BYTES, bar);
+    for (int i = 0; i < BATCH / 32; i++) {
+        const int j = i * 32 + lane;
+        if (j < n) {
+            const char* src = reinterpret_cast<const char*>(recs + id[i]);
+            const uint32_t dst = s_rec + j * REC_BYTES;
+            asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
+            asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst + 16), "l"(src + 16) : "memory");
+            asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst + 32), "l"(src + 32) : "memory");
         }
-    } else {
-#pragma unroll
-        for (int i = 0; i < BATCH / 32; i++) {
-            const int j = i * 32 + lane;
-            if (j < n) {
-                const char* src = reinterpret_cast<const char*>(recs + id[i]);
-                const uint32_t dst = s_rec + j * REC_BYTES;
-                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
-                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst + 16), "l"(src + 16) : "memory");
-                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst + 32), "l"(src + 32) : "memory");
-            }
-        }
-        if (KEEP_IDS) __threadfence_block();        // the ids written above must be visible to whoever sees the stage complete
-        asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
     }
+    if (KEEP_IDS) __threadfence_block();        // the ids written above must be visible to whoever sees the stage complete
+    asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
 }
-constexpr uint32_t full_count(bool tma) { return tma ? 1u : 32u; }
 __device__ __forceinline__ void mbar_arrive_n(uint32_t bar, uint32_t n) {
     asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0], %1;\n\t}" ::"r"(bar), "r"(n) : "memory");
 }
@@ -276,29 +255,7 @@ __device__ __forceinline__ bool fwd_live(float p, float al) { return (p <= 0.f) 
 
 struct FwdAcc { float c0a, c0b, c1a, c1b, c2a, c2b, da, db, aa, ab; };
 
-__device__ __forceinline__ void fwd_back(const FwdFront& f, bool liveA, bool liveB, uint32_t ra, uint32_t pos, float& TA,
-                                         float& TB, FwdAcc& acc, uint32_t& lastA, uint32_t& lastB,
-                                         float& pyfA, float& pyfB) {
-    const u64 T2 = pk(TA, TB);
-    const u64 tt2 = mul2(T2, sub2(bc(1.f), f.al2));          // T * (1 - alpha)
-    const bool stopA = liveA && (lo(tt2) < 0.0001f), stopB = liveB && (hi(tt2) < 0.0001f);
-    const bool blA = liveA && !stopA, blB = liveB && !stopB;
-    const u64 w2raw = mul2(f.al2, T2);
-    const u64 w2 = pk(blA ? lo(w2raw) : 0.f, blB ? hi(w2raw) : 0.f);
-    const float4 k = lds128(ra + 32);
-    u64 t;
-    t = fma2(bc(k.x), w2, pk(acc.c0a, acc.c0b)); acc.c0a = lo(t); acc.c0b = hi(t);
-    t = fma2(bc(k.y), w2, pk(acc.c1a, acc.c1b)); acc.c1a = lo(t); acc.c1b = hi(t);
-    t = fma2(bc(k.z), w2, pk(acc.c2a, acc.c2b)); acc.c2a = lo(t); acc.c2b = hi(t);
-    t = fma2(bc(f.gz), w2, pk(acc.da, acc.db)); acc.da = lo(t); acc.db = hi(t);
-    t = add2(pk(acc.aa, acc.ab), w2); acc.aa = lo(t); acc.ab = hi(t);
-    TA = blA ? lo(tt2) : TA; TB = blB ? hi(tt2) : TB;
-    lastA = blA ? pos : lastA; lastB = blB ? pos : lastB;
-    const float QNAN = __int_as_float(0x7fc00000);           // terminated: the pixel's row coordinate becomes NaN
-    pyfA = stopA ? QNAN : pyfA; pyfB = stopB ? QNAN : pyfB;
-}
-
-// Variant of fwd_back for the common case "no pixel of the warp terminates at this visit": a pixel that does not take
+// The blend, written for the common case "no pixel of the warp terminates at this visit": a pixel that does not take
 // the splat blends it with alpha 0 (T * (1 - 0) = T exactly, weight 0), so T and the weights need no per-pixel
 // selects; T stays >= 1e-4 for every pixel that has not terminated, hence "T (1 - alpha) < 1e-4" alone identifies a
 // terminating pixel and ONE warp vote per visit guards the fix-up (weight 0, T kept, row coordinate poisoned).
@@ -332,18 +289,25 @@ __device__ __forceinline__ void fwd_back_sv(const FwdFront& f, bool liveA, bool 
     t = add2(pk(acc.aa, acc.ab), w2); acc.aa = lo(t); acc.ab = hi(t);
 }
 
+// Ring depth of the forward: three 6 KB stages of static shared memory (two and four were no faster, DESIGN.md 5.1).
+constexpr int FWD_RING_STAGES = 3;
+// The shipped backward: ring depth, queued visits per flush, CTAs per SM.  2 x 6 KB ring + 20 KB partial block + 34 KB
+// queue + 4 KB upstream gradients = 70.4 KB, three CTAs per SM (an H100 SM has 228 KB of shared memory and reserves
+// 1 KB per CTA).  Measured on an H100 against one partial block per stage (92.6 KB, two CTAs per SM): 0.654-0.661
+// against 0.739 ms per config-1 view.  A third ring stage would take 76.5 KB and fall back to two CTAs per SM.
+constexpr int BWD_STAGES = 2, BWD_SLOTS = 16, BWD_MINB = 3;
+
 // =================================================================================================
 // forward
 // =================================================================================================
-template <int STAGES, bool TMA, bool STOPVOTE>
 __global__ void __launch_bounds__(NTHREADS)
 composite_forward_kernel(ViewArgs va, const SplatRec* __restrict__ recs, const uint32_t* __restrict__ point_list,
                          const uint32_t* __restrict__ ranges, float* __restrict__ out_color,
                          float* __restrict__ out_depth, float* __restrict__ out_alpha,
                          uint32_t* __restrict__ n_contrib, float* __restrict__ final_T) {
-    __shared__ __align__(128) unsigned char s_rec_raw[STAGES * STAGE_BYTES];
-    __shared__ __align__(8) u64 s_full[STAGES];
-    __shared__ uint32_t s_cnt[STAGES], s_stop;
+    __shared__ __align__(128) unsigned char s_rec_raw[FWD_RING_STAGES * STAGE_BYTES];
+    __shared__ __align__(8) u64 s_full[FWD_RING_STAGES];
+    __shared__ uint32_t s_cnt[FWD_RING_STAGES], s_stop;
     const uint32_t s_rec = (uint32_t)__cvta_generic_to_shared(s_rec_raw);
     const uint32_t a_full = (uint32_t)__cvta_generic_to_shared(s_full);
     const uint32_t a_stop = (uint32_t)__cvta_generic_to_shared(&s_stop);
@@ -354,14 +318,14 @@ composite_forward_kernel(ViewArgs va, const SplatRec* __restrict__ recs, const u
     const int nb = (len + BATCH - 1) / BATCH;
 
     if (tid == 0) {
-        for (int i = 0; i < STAGES; i++) { mbar_init(a_full + 8 * i, full_count(TMA)); s_cnt[i] = 0; }
+        for (int i = 0; i < FWD_RING_STAGES; i++) { mbar_init(a_full + 8 * i, STAGE_ARRIVALS); s_cnt[i] = 0; }
         s_stop = 0xFFFFFFFFu;
         mbar_fence_init();
     }
     __syncthreads();
     // first fill of the ring: warp w gathers batch w (afterwards the LAST warp to finish a stage refills it)
-    if (warp < STAGES && warp < nb)
-        produce_stage<false, TMA>(recs, point_list + start + warp * BATCH, min(BATCH, len - warp * BATCH), s_rec + warp * STAGE_BYTES, 0u,
+    if (warp < FWD_RING_STAGES && warp < nb)
+        produce_stage<false>(recs, point_list + start + warp * BATCH, min(BATCH, len - warp * BATCH), s_rec + warp * STAGE_BYTES, 0u,
                              a_full + 8 * warp, lane);
 
     const int X0 = blockIdx.x * GS_TILE + 8 * (warp & 1), Y0 = blockIdx.y * GS_TILE + 8 * (warp >> 1);
@@ -406,47 +370,40 @@ composite_forward_kernel(ViewArgs va, const SplatRec* __restrict__ recs, const u
                     const FwdFront f1 = fwd_front(ra1, pxf, pyfA, pyfB);
                     // (no warp vote around the blend: 96 % of the visits have a live lane, and the branch made ptxas copy
                     // the ten accumulator registers at its join)
-                    if (STOPVOTE) {
-                        fwd_back_sv(f0, fwd_live(lo(f0.p2), lo(f0.al2)), fwd_live(hi(f0.p2), hi(f0.al2)), ra0, pos0 + j0,
-                                    TA, TB, acc, lastA, lastB, pyfA, pyfB);
-                        fwd_back_sv(f1, two && fwd_live(lo(f1.p2), lo(f1.al2)) && (pyfA == pyfA), two && fwd_live(hi(f1.p2), hi(f1.al2)) && (pyfB == pyfB),
-                                    ra1, pos0 + j1, TA, TB, acc, lastA, lastB, pyfA, pyfB);
-                        continue;
-                    }
-                    fwd_back(f0, fwd_live(lo(f0.p2), lo(f0.al2)), fwd_live(hi(f0.p2), hi(f0.al2)), ra0, pos0 + j0,
-                             TA, TB, acc, lastA, lastB, pyfA, pyfB);
+                    fwd_back_sv(f0, fwd_live(lo(f0.p2), lo(f0.al2)), fwd_live(hi(f0.p2), hi(f0.al2)), ra0, pos0 + j0,
+                                TA, TB, acc, lastA, lastB, pyfA, pyfB);
                     // visit 1's front half saw the row coordinates from before visit 0: drop pixels that just terminated
                     // (`two` false: j1 == j0 and the visit is masked off as a whole)
-                    fwd_back(f1, two && fwd_live(lo(f1.p2), lo(f1.al2)) && (pyfA == pyfA), two && fwd_live(hi(f1.p2), hi(f1.al2)) && (pyfB == pyfB),
-                             ra1, pos0 + j1, TA, TB, acc, lastA, lastB, pyfA, pyfB);
+                    fwd_back_sv(f1, two && fwd_live(lo(f1.p2), lo(f1.al2)) && (pyfA == pyfA), two && fwd_live(hi(f1.p2), hi(f1.al2)) && (pyfB == pyfB),
+                                ra1, pos0 + j1, TA, TB, acc, lastA, lastB, pyfA, pyfB);
                 }
                 if (__all_sync(0xFFFFFFFFu, (pyfA != pyfA) && (pyfB != pyfB))) { warp_done = true; break; }
             }
         }
-        // release the stage; the last of the four warps to do so refills it with batch b + STAGES.  Each release carries
-        // the warp's "all my pixels have terminated" bit: when all four say so the tile is finished, nothing is gathered
-        // any more and the stop batch is published (a function of b only, so concurrent refills cannot disagree).
+        // release the stage; the last of the four warps to do so refills it with batch b + FWD_RING_STAGES.  Each release
+        // carries the warp's "all my pixels have terminated" bit: when all four say so the tile is finished, nothing is
+        // gathered any more and the stop batch is published (a function of b only, so concurrent refills cannot disagree).
         __syncwarp();
         uint32_t tot = 0;
         if (lane == 0) { __threadfence_block(); tot = atomicAdd(&s_cnt[rs.stage], 1u + (warp_done ? 0x100u : 0u)) + 1u + (warp_done ? 0x100u : 0u); }
         tot = __shfl_sync(0xFFFFFFFFu, tot, 0);
         if ((tot & 0xFFu) == NMATH) {
-            const int nbatch = b + STAGES;
+            const int nbatch = b + FWD_RING_STAGES;
             // acquire side of the hand-over (release = the fence before each warp's atomic): the other warps' reads of
             // the stage happen before the refill below overwrites it
             if (lane == 0) { __threadfence_block(); s_cnt[rs.stage] = 0; }
             __syncwarp();
             if (nbatch < nb) {
                 if ((tot >> 8) == NMATH) {
-                    if (lane == 0) { atomicMin(&s_stop, (uint32_t)nbatch); __threadfence_block(); mbar_arrive_n(a_full + 8 * rs.stage, full_count(TMA)); }
+                    if (lane == 0) { atomicMin(&s_stop, (uint32_t)nbatch); __threadfence_block(); mbar_arrive_n(a_full + 8 * rs.stage, STAGE_ARRIVALS); }
                 } else {
                     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // the stage was read through the generic proxy
-                    produce_stage<false, TMA>(recs, point_list + start + nbatch * BATCH, min(BATCH, len - nbatch * BATCH),
+                    produce_stage<false>(recs, point_list + start + nbatch * BATCH, min(BATCH, len - nbatch * BATCH),
                                          s_rec + rs.stage * STAGE_BYTES, 0u, a_full + 8 * rs.stage, lane);
                 }
             }
         }
-        rs.advance(STAGES);
+        rs.advance(FWD_RING_STAGES);
     }
     const size_t plane = (size_t)va.W * va.H;
     const float bg0 = __ldg(va.bg), bg1 = __ldg(va.bg + 1), bg2 = __ldg(va.bg + 2);
@@ -684,7 +641,7 @@ composite_backward_kernel(ViewArgs va, const SplatRec* __restrict__ recs, const 
     for (int o = 16; o > 0; o >>= 1) wmax = max(wmax, __shfl_xor_sync(0xFFFFFFFFu, wmax, o));
     if (lane == 0) s_wmax[warp] = wmax;
     if (tid == 0) {
-        for (int i = 0; i < STAGES; i++) { mbar_init(a_full + 8 * i, full_count(false)); s_cnt[i] = 0; }
+        for (int i = 0; i < STAGES; i++) { mbar_init(a_full + 8 * i, STAGE_ARRIVALS); s_cnt[i] = 0; }
         mbar_init(a_free, 1);
         mbar_fence_init();
     }
@@ -696,8 +653,8 @@ composite_backward_kernel(ViewArgs va, const SplatRec* __restrict__ recs, const 
     // stages are gathered from the back of the list: iteration `it` holds list positions [(nb-1-it)*BATCH, +BATCH)
     auto produce = [&](int it, uint32_t stage) {
         const int base = (nb - 1 - it) * BATCH;
-        produce_stage<false, false>(recs, point_list + start + base, min(BATCH, (int)nproc - base), s_rec + stage * STAGE_BYTES,
-                                    0u, a_full + 8 * stage, lane);
+        produce_stage<false>(recs, point_list + start + base, min(BATCH, (int)nproc - base), s_rec + stage * STAGE_BYTES,
+                             0u, a_full + 8 * stage, lane);
     };
     if (warp < STAGES && warp < nb) produce(warp, warp);       // first fill; afterwards the last warp to finish a stage refills it
 
@@ -805,11 +762,6 @@ constexpr size_t bwd_smem_bytes(int stages, int slots) {
            NMATH * 64 * 16 + NMATH * (size_t)slots * 4 + 8 * (size_t)stages + 8 + 4 * (size_t)stages + 16;
 }
 
-// The shipped backward: ring depth, queued visits per flush, CTAs per SM.  2 x 6 KB ring + 20 KB partial block + 34 KB
-// queue + 4 KB upstream gradients = 70.4 KB, three CTAs per SM (an H100 SM has 228 KB of shared memory and reserves
-// 1 KB per CTA).  Measured on an H100 against one partial block per stage (92.6 KB, two CTAs per SM): 0.654-0.661
-// against 0.739 ms per config-1 view.  A third ring stage would take 76.5 KB and fall back to two CTAs per SM.
-constexpr int BWD_STAGES = 2, BWD_SLOTS = 16, BWD_MINB = 3;
 constexpr size_t BWD_SMEM = bwd_smem_bytes(BWD_STAGES, BWD_SLOTS);
 static_assert(BWD_MINB * (BWD_SMEM + 1024) <= 228 * 1024, "the backward's shared memory must fit BWD_MINB CTAs per SM");
 #define BWD_KERNEL composite_backward_kernel<BWD_STAGES, BWD_SLOTS, BWD_MINB>
@@ -826,52 +778,14 @@ cudaError_t bwd_kernel_attributes() {
     return err;
 }
 
-bool gather_tma() {       // GS_B200_GATHER=tma selects the TMA bulk-copy gather instead of the cp.async default
-    static const bool tma = []() { const char* e = getenv("GS_B200_GATHER"); return e && e[0] == 't'; }();
-    return tma;
-}
-
-int env_int(const char* name, int dflt) {
-    const char* e = getenv(name);
-    return (e && *e) ? atoi(e) : dflt;
-}
-
 }  // namespace
-
-// round-1 kernels (gs_render.cu), kept selectable for A/B measurements: GS_B200_COMPOSITE=r1
-int gs_launch_render_forward_r1(const ViewArgs& va, const SplatRec* recs, const uint32_t* point_list,
-                                const uint32_t* ranges, float* out_color, float* out_depth, float* out_alpha,
-                                uint32_t* n_contrib, float* final_T, cudaStream_t s);
-int gs_launch_render_backward_r1(const ViewArgs& va, const SplatRec* recs, const uint32_t* point_list,
-                                 const uint32_t* ranges, const uint32_t* n_contrib, const float* final_T,
-                                 const float* dL_dcolor, const float* dL_ddepth, const float* dL_dalpha,
-                                 SplatGrad* sg, cudaStream_t s);
-
-#include <atomic>
-static std::atomic<int> g_composite_mode{[]() { const char* e = getenv("GS_B200_COMPOSITE"); return (e && e[0] == 'r') ? 1 : 0; }()};
-static bool use_r1() { return g_composite_mode.load(std::memory_order_relaxed) == 1; }
-extern "C" int32_t gs_b200_debug_set_composite(int32_t mode) {
-    if (mode != 0 && mode != 1) { gs_set_error("composite mode must be 0 (round-2 kernels) or 1 (round-1 kernels)"); return 1; }
-    g_composite_mode.store(mode);
-    return 0;
-}
 
 int gs_launch_render_forward(const ViewArgs& va, const SplatRec* recs, const uint32_t* point_list,
                              const uint32_t* ranges, float* out_color, float* out_depth, float* out_alpha,
                              uint32_t* n_contrib, float* final_T, cudaStream_t s) {
-    if (use_r1()) return gs_launch_render_forward_r1(va, recs, point_list, ranges, out_color, out_depth, out_alpha, n_contrib, final_T, s);
     dim3 grid(va.tiles_x, va.tiles_y);
-    // ring depth: GS_B200_FWD_STAGES (2/3/4, cp.async gather); the TMA gather (GS_B200_GATHER=tma) is kept at its best
-    // measured depth for A/B runs
-    static const int stages = env_int("GS_B200_FWD_STAGES", 3);
-    static const bool stopvote = env_int("GS_B200_FWD_STOPVOTE", 1) != 0;   // one warp vote per visit instead of per-pixel termination selects
-#define FWD(ST, TM, SV) composite_forward_kernel<ST, TM, SV><<<grid, NTHREADS, 0, s>>>(va, recs, point_list, ranges, out_color, out_depth, out_alpha, n_contrib, final_T)
-    if (gather_tma()) FWD(3, true, false);
-    else if (stages == 2) FWD(2, false, false);
-    else if (stages == 4) FWD(4, false, false);
-    else if (stopvote) FWD(3, false, true);
-    else FWD(3, false, false);
-#undef FWD
+    composite_forward_kernel<<<grid, NTHREADS, 0, s>>>(va, recs, point_list, ranges, out_color, out_depth, out_alpha,
+                                                       n_contrib, final_T);
     gs_count_launches(1);
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
@@ -881,7 +795,6 @@ int gs_launch_render_backward(const ViewArgs& va, const SplatRec* recs, const ui
                               const uint32_t* ranges, const uint32_t* n_contrib, const float* final_T,
                               const float* dL_dcolor, const float* dL_ddepth, const float* dL_dalpha,
                               SplatGrad* sg, cudaStream_t s) {
-    if (use_r1()) return gs_launch_render_backward_r1(va, recs, point_list, ranges, n_contrib, final_T, dL_dcolor, dL_ddepth, dL_dalpha, sg, s);
     dim3 grid(va.tiles_x, va.tiles_y);
     GS_CUDA_CHECK(bwd_kernel_attributes());
     BWD_KERNEL<<<grid, NTHREADS, BWD_SMEM, s>>>(va, recs, point_list, ranges, n_contrib, final_T, dL_dcolor, dL_ddepth,

@@ -185,8 +185,7 @@ __global__ void __launch_bounds__(128) knn_search_kernel(const float4* __restric
 int gs_launch_knn(const float* points, int N, float* out, cudaStream_t s) {
     if (N <= 0) return 0;
     if (!points || !out) { gs_set_error("knn: NULL"); return 1; }
-    static const bool force_allpairs = []() { const char* e = getenv("GS_B200_KNN_ALLPAIRS"); return e && e[0] == '1'; }();
-    if (N < 8192 || force_allpairs) {
+    if (N < 8192) {
         knn3_kernel<<<(N + KT - 1) / KT, KT, 0, s>>>(points, N, out);
         gs_count_launches(1);
         GS_CUDA_CHECK(cudaGetLastError());

@@ -360,13 +360,11 @@ int ngp_grid_encode_bwd(const float* x, long long N, const int32_t* offsets_host
                         const float* g_out, float* d_emb, cudaStream_t s) {
     if (N <= 0) return 0;
     GridMeta gm; if (make_meta(gm, offsets_host, L, bound, pls, base)) return 1;
-    static const bool v4env = []() { const char* e = getenv("NGP_B200_RED_V4"); return !(e && e[0] == '0'); }();
-    static const bool runs = []() { const char* e = getenv("NGP_B200_BWD_RUNS"); return !(e && e[0] == '0'); }();
-    const bool v4 = v4env && ((uintptr_t)d_emb & 15) == 0;
+    const bool v4 = ((uintptr_t)d_emb & 15) == 0;
     // coarse levels (resolution <= 128: runs of >= ~3 samples per cell at the reference's 5e-3 step) go through the
     // run-reducing kernel; they are the first levels since resolutions grow with the level index
     int l0 = 0;
-    if (runs) while (l0 < L && gm.res[l0] <= 128 && l0 < 8) l0++;
+    while (l0 < L && gm.res[l0] <= 128 && l0 < 8) l0++;
     if (l0 > 0) {
         const dim3 grid((unsigned)((N + 255) / 256), (unsigned)l0);
         if (v4) grid_encode_bwd_runs_kernel<true><<<grid, 256, 0, s>>>(x, N, gm, (const float2*)g_out, (float2*)d_emb);

@@ -178,12 +178,10 @@ lib.gs_b200_get_tile_culling.argtypes = []
 GRAD_SINK = C.CFUNCTYPE(None, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p)
 lib.gs_b200_set_grad_sink.restype = _I
 lib.gs_b200_set_grad_sink.argtypes = [GRAD_SINK, _P, _I]
-lib.gs_b200_debug_set_composite.restype = _I
-lib.gs_b200_debug_set_composite.argtypes = [_I]
 lib.gs_b200_composite_bwd_occupancy.restype = _I
 lib.gs_b200_composite_bwd_occupancy.argtypes = [C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
 
-EXPORTS = ["gs_b200_set_grad_sink", "gs_b200_debug_set_composite", "gs_b200_composite_bwd_occupancy", "gs_b200_image_loss", "gs_b200_step_device_train", "gs_b200_step_device_hook", "gs_b200_render_views", "gs_b200_set_tile_culling", "gs_b200_get_tile_culling", "gs_b200_step_device", "gs_b200_step_host_dev_grads", "gs_b200_launch_count", "gs_b200_profile_enable", "gs_b200_profile_read",
+EXPORTS = ["gs_b200_set_grad_sink", "gs_b200_composite_bwd_occupancy", "gs_b200_image_loss", "gs_b200_step_device_train", "gs_b200_step_device_hook", "gs_b200_render_views", "gs_b200_set_tile_culling", "gs_b200_get_tile_culling", "gs_b200_step_device", "gs_b200_step_host_dev_grads", "gs_b200_launch_count", "gs_b200_profile_enable", "gs_b200_profile_read",
            "gs_b200_abi_version", "gs_b200_last_error", "gs_b200_rasterize_forward", "gs_b200_rasterize_backward",
            "gs_b200_state_free", "gs_b200_debug_sorted_keys", "gs_b200_sort_scratch_bytes",
            "gs_b200_sort_pairs_u32", "gs_b200_knn_mean_dist2", "gs_b200_step_host"]

@@ -92,13 +92,7 @@ const char* gs_b200_last_error(void);
 int32_t gs_b200_set_tile_culling(int32_t mode);
 int32_t gs_b200_get_tile_culling(void);
 
-/* Measurement switch (no reference counterpart): which tile-composite kernels run.  0 (default): the round-2
- * kernels (gs_composite.cu: two pixels per lane, cp.async-fed mbarrier ring, queued gradient phase, fp64 gradient sums);
- * 1: the round-1 kernels (gs_render.cu), kept for A/B timing.  Results agree (images bit for bit).
- * Initial value from the environment variable GS_B200_COMPOSITE ("r1" selects 1). */
-int32_t gs_b200_debug_set_composite(int32_t mode);
-
-/* Measurement query (no reference counterpart): CTAs per SM of the round-2 composite backward kernel as the CUDA
+/* Measurement query (no reference counterpart): CTAs per SM of the composite backward kernel as the CUDA
  * occupancy calculator reports it for the current device, with the kernel's launch attributes applied, and the
  * kernel's dynamic shared memory per CTA in bytes. */
 int32_t gs_b200_composite_bwd_occupancy(int32_t* ctas_per_sm, int32_t* smem_bytes);
@@ -181,7 +175,6 @@ int32_t gs_b200_step_device(
  * Upload order: views, geometry parameters, SH block, upstream gradients view by view.  For V <= 8 the step starts
  * as soon as the geometry is resident (projection, sorting and binning of every view need nothing else) and fills the
  * colours into the records when the SH block has landed; images are bit-identical to gs_b200_step_device.
- * GS_B200_HOST_LATE_SH=0 in the environment makes it wait for the whole upload first.
  */
 int32_t gs_b200_step_host(
     int32_t V, int32_t H, int32_t W, int32_t sh_degree, float scale_modifier, const float* views_host,

@@ -1,8 +1,8 @@
 """Composite kernels against a float64 evaluation of the same operation, on scenes built in pixel units at the edges
 where the kernels go wrong: tile lists of exactly L records around the 128-record ring stages (S1), pixels that
 terminate at chosen list positions (S2), large thin rotated splats whose alpha = 1/255 level set crosses quadrant
-corners and tile rows (S3), and frames whose edge tiles are mostly outside the image (S4).  The forward's selectable
-variants, the round-1 kernels and the library's other measurement switches are run on the same scenes or workloads.
+corners and tile rows (S3), and frames whose edge tiles are mostly outside the image (S4).  Two runs of the same scenes
+in one process must agree bit for bit.
 
 Reference.  `oracle/gs_oracle.py`'s composite in float64, run on the records the kernels work on: the fp32 oracle's
 preprocess outputs (which reproduce the library's; its integer outputs are checked bit for bit) cast to double.  The
@@ -28,19 +28,13 @@ gradients, so every gradient is also held to GRAD_REL (1e-4) norm- and element-r
 suite's 1e-3, and every image error to IMG_CAP (3e-5), whichever bar is smaller.  The test prints each bar's size, the
 worst error / bar ratio and the worst error per quantity."""
 import math
-import os
-import subprocess
-import sys
 from functools import lru_cache
 
 import numpy as np
 import pytest
 import torch
 
-if __name__ == "__main__":          # child process (see the end of the file): the package and the oracle from this tree
-    _root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    sys.path[:0] = [os.path.join(_root, "comfyui-3d-pack_b200"), _root]
-from oracle import gs_oracle as O  # noqa: E402
+from oracle import gs_oracle as O
 
 NAMES = ("means3D", "shs", "opacities", "scales", "rotations")
 GRADS = NAMES + ("means2D",)
@@ -511,20 +505,13 @@ def dev():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("kernels", ["r2", "r1"])
 @pytest.mark.parametrize("name", SCENES)
-def test_scene_matches_fp64(dev, name, kernels):
-    """round-2 (shipped) and round-1 composite kernels, one scene, against the fp64 bars"""
-    from gs_b200 import _lib
+def test_scene_matches_fp64(dev, name):
+    """the composite kernels, one scene, against the fp64 bars"""
     r = reference(name)
-    if kernels == "r1":
-        _lib.check(_lib.lib.gs_b200_debug_set_composite(1))
-    try:
-        got = kernel_outputs(r["cl"], r["st"], r["up"], dev)
-    finally:
-        _lib.check(_lib.lib.gs_b200_debug_set_composite(0))
+    got = kernel_outputs(r["cl"], r["st"], r["up"], dev)
     worst = check_against_fp64(name, got)
-    print(f"{name} {kernels}: excluded {int(r['an']['excluded'].sum())} px; worst " +
+    print(f"{name}: excluded {int(r['an']['excluded'].sum())} px; worst " +
           " ".join(f"{k}={v:.3g}" for k, v in worst.items()))
 
 
@@ -684,145 +671,23 @@ def test_s3_every_pixel_above_the_level_set_shows_the_splat(dev, culling):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# the forward's selectable variants and the round-1 kernels on the same scenes (child processes: the switches are read
-# once per process)
+# run-to-run determinism on the scenes above
 # ---------------------------------------------------------------------------------------------------------------------
-# composite_forward_kernel<STAGES, TMA, STOPVOTE> differs between variants only in the gather (cp.async or one bulk copy
-# per record, same bytes), the ring depth (which stage a batch lands in and when it is refilled), and the termination
-# update (per-pixel selects, or one warp vote per visit): fwd_back_sv blends a non-live pixel with alpha 0, which leaves
-# T, the weight (0) and the accumulators bit-identical to the select of fwd_back, and it identifies a stopping pixel by
-# T (1 - alpha) < 1e-4 alone, which only a live pixel can reach (T >= 1e-4 otherwise).  The per-visit arithmetic and
-# its order are the same in all of them, so every output and the resulting gradients are expected bit-identical.
-VARIANTS = {"stages2": {"GS_B200_FWD_STAGES": "2"}, "stages4": {"GS_B200_FWD_STAGES": "4"},
-            "stopvote0": {"GS_B200_FWD_STOPVOTE": "0"}, "tma": {"GS_B200_GATHER": "tma"}}
-SWITCH_ENV = ("GS_B200_FWD_STAGES", "GS_B200_FWD_STOPVOTE", "GS_B200_GATHER", "GS_B200_COMPOSITE", "GS_B200_STEP_OVERLAP",
-              "GS_B200_HOST_LATE_SH", "GS_B200_KNN_ALLPAIRS", "NGP_B200_RED_V4", "NGP_B200_BWD_RUNS", "GS_B200_TILE_CULLING")
-VARIANT_SCENES = ["S1", "S2u128", "S2u257", "S2q0", "S2q1", "S417x33", "S42000x16"]
-
-
-def _child(mode, out, env_extra):
-    env = {k: v for k, v in os.environ.items() if k not in SWITCH_ENV}
-    env.update(env_extra, PYTHONNOUSERSITE="1")
-    subprocess.run([sys.executable, os.path.abspath(__file__), mode, str(out)], check=True, env=env, timeout=900)
-    return dict(np.load(out))
+REPEAT_SCENES = ["S1", "S2u128", "S2u257", "S2q0", "S2q1", "S417x33", "S42000x16"]
 
 
 def _scene_outputs(dev):
     res = {}
-    for name in VARIANT_SCENES:
+    for name in REPEAT_SCENES:
         cl, st, up = scene(name)
         for k, v in kernel_outputs(cl, st, up, dev).items():
             res[f"{name}/{k}"] = v.numpy()
     return res
 
 
-@pytest.fixture(scope="module")
-def default_child(tmp_path_factory):
-    return _child("scenes", tmp_path_factory.mktemp("default") / "out.npz", {})
-
-
 @pytest.mark.gpu
-def test_default_runs_are_bit_identical(default_child):
-    """the default child runs every scene twice and stores both"""
-    for k in default_child:
-        if k.startswith("again/"):
-            assert np.array_equal(default_child[k], default_child[k[6:]], equal_nan=True), k
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("variant", sorted(VARIANTS))
-def test_forward_variant_is_bit_identical(default_child, tmp_path, variant):
-    got = _child("scenes", tmp_path / "out.npz", VARIANTS[variant])
-    diff = [k for k in default_child if not k.startswith("again/") and not np.array_equal(got[k], default_child[k], equal_nan=True)]
-    assert not diff, f"{variant}: differs from the default in {diff[:10]}"
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# the remaining measurement switches, once each, on workloads of the existing tests
-# ---------------------------------------------------------------------------------------------------------------------
-def _workload(kind, dev):
-    from gs_b200 import camera, optim_step, synthetic
-    if kind == "overlap":        # the multi-view step (7 views: the overlap cuts steps of >= 6 views into two chunks)
-        N, V, W, H, deg = 20000, 7, 256, 144, 2
-        params = optim_step.PackedParams(synthetic.make_cloud("D1", N, deg, seed=5, device=dev))
-        views = optim_step.ViewSet(camera.orbit_views(V, W, H), W, H, deg, dev)
-        dl = (torch.rand(V, 5, H, W, generator=torch.Generator().manual_seed(7)) * 2 - 1).to(dev)
-        img = torch.empty(V, 5, H, W, device=dev)
-        pairs = optim_step.step_device_pipelined(params, views, dl, img)
-        torch.cuda.synchronize()
-        return {"images": img.cpu().numpy(), "grads": params.grads.cpu().numpy(), "pairs": np.array(pairs)}
-    if kind == "late_sh":        # the host-buffer step
-        N, V, W, H, deg = 30000, 4, 320, 176, 3
-        cloud = synthetic.make_cloud("D1", N, deg, seed=9, device=dev)
-        vnp = camera.orbit_views(V, W, H)
-        dl = torch.rand(V, 5, H, W, generator=torch.Generator().manual_seed(3)) * 2 - 1
-        hs = optim_step.HostStep({k: v.cpu() for k, v in cloud.items()}, vnp, W, H, deg, dl)
-        img = torch.empty(V, 5, H, W).pin_memory()
-        pairs = hs.run(images=img)
-        return {"images": img.clone().numpy(), "grads": hs.grads.clone().numpy(), "pairs": np.array(pairs)}
-    if kind == "knn":            # the kd-tree check, above the all-pairs size
-        from gs_b200 import rasterizer as R
-        g = torch.Generator().manual_seed(40000)
-        c = torch.rand(20, 3, generator=g) * 4 - 2
-        n = 40000
-        pts = torch.cat([c[torch.randint(0, 20, (n - 500,), generator=g)] + 0.01 * torch.randn(n - 500, 3, generator=g),
-                         torch.rand(500, 3, generator=g) * 20 - 10]).float().contiguous()
-        ball = O.make_cloud("D0", 60000, 0, seed=2)["means3D"].contiguous()
-        return {"pts_clusters": pts.numpy(), "clusters": R.knn_mean_dist2(pts.to(dev)).cpu().numpy(),
-                "pts_ball": ball.numpy(), "ball": R.knn_mean_dist2(ball.to(dev)).cpu().numpy()}
-    if kind == "grid":           # the hash-grid forward / backward
-        from kiui.gridencoder import GridEncoder
-        torch.manual_seed(16)
-        enc = GridEncoder(num_levels=16).to(dev)
-        enc.embeddings.data.uniform_(-1, 1)
-        x = torch.rand(5000, 3) * 2 - 1
-        x[:4] = torch.tensor([[-1.0, -1, -1], [1, 1, 1], [0, 0, 0], [1, -1, 0.5]])
-        gout = torch.rand(5000, 32)
-        emb = enc.embeddings.detach().cpu().clone()
-        out = enc(x.to(dev))
-        (out * gout.to(dev)).sum().backward()
-        torch.cuda.synchronize()
-        return {"x": x.numpy(), "gout": gout.numpy(), "emb": emb.numpy(), "out": out.detach().cpu().numpy(),
-                "grad": enc.embeddings.grad.cpu().numpy()}
-    raise ValueError(kind)
-
-
-SWITCHES = [("overlap", {"GS_B200_STEP_OVERLAP": "1"}), ("late_sh", {"GS_B200_HOST_LATE_SH": "0"}),
-            ("knn", {"GS_B200_KNN_ALLPAIRS": "1"}), ("grid", {"NGP_B200_RED_V4": "0"}), ("grid", {"NGP_B200_BWD_RUNS": "0"})]
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("kind,env", SWITCHES, ids=[list(e)[0] for _, e in SWITCHES])
-def test_measurement_switch(dev, tmp_path, kind, env):
-    """images bit-identical where the code claims it (the step entries), gradients to the summation-order bar of the
-    existing tests (1e-5 relative); kNN and the hash grid against their oracles with the existing bars"""
-    got = _child("workload:" + kind, tmp_path / "out.npz", env)
-    if kind in ("overlap", "late_sh"):
-        ref = _workload(kind, dev)
-        assert int(got["pairs"]) == int(ref["pairs"])
-        assert np.array_equal(got["images"], ref["images"])
-        g, r = got["grads"].astype(np.float64), ref["grads"].astype(np.float64)
-        assert np.linalg.norm(g - r) / np.linalg.norm(r) < 1e-5
-    elif kind == "knn":
-        for k in ("clusters", "ball"):
-            assert np.allclose(got[k], O.knn_mean_dist2(got["pts_" + k]), rtol=1e-4, atol=1e-9), k
-    else:
-        from oracle import ngp_oracle as G
-        off = G.grid_offsets(num_levels=16)
-        x, emb, gout = (torch.from_numpy(got[k]) for k in ("x", "emb", "gout"))
-        assert float(np.abs(got["out"] - G.grid_encode(x, emb, off, num_levels=16).numpy()).max()) < 2e-5
-        e = emb.clone().requires_grad_(True)
-        (G.grid_encode(x, e, off, num_levels=16) * gout).sum().backward()
-        ref = e.grad.double()
-        assert float((torch.from_numpy(got["grad"]).double() - ref).norm() / ref.norm()) < 1e-5
-
-
-if __name__ == "__main__":          # child process: one switch setting per process
-    mode, path = sys.argv[1], sys.argv[2]
-    d = torch.device("cuda:0")
-    if mode == "scenes":
-        res = _scene_outputs(d)
-        res.update({"again/" + k: v for k, v in _scene_outputs(d).items()})
-    else:
-        res = _workload(mode.split(":", 1)[1], d)
-    np.savez(path, **res)
+def test_default_runs_are_bit_identical(dev):
+    """every output and gradient of the scenes, run twice in one process, is bit-identical"""
+    first, again = _scene_outputs(dev), _scene_outputs(dev)
+    for k in first:
+        assert np.array_equal(first[k], again[k], equal_nan=True), k
