@@ -184,7 +184,12 @@ def _mip_level(uv_da, Ht, Wt, n_levels, mip_level_bias=None):
     A = dsdx * dsdx + dtdx * dtdx
     Bq = dsdy * dsdy + dtdy * dtdy
     Cq = dsdx * dsdy + dtdx * dtdy
-    major2 = 0.5 * (A + Bq) + torch.sqrt(0.25 * (A - Bq) * (A - Bq) + Cq * Cq)
+    r2 = 0.25 * (A - Bq) * (A - Bq) + Cq * Cq
+    # sqrt guarded at 0 (every isotropic footprint, and uv_da = 0): same value, and the root's subgradient 0 there instead
+    # of sqrt's infinite derivative (which made d uv_da NaN); along any direction the gradient is then the mean of the
+    # two one-sided derivatives
+    pos_r2 = r2 > 0
+    major2 = 0.5 * (A + Bq) + torch.where(pos_r2, torch.sqrt(torch.where(pos_r2, r2, torch.ones_like(r2))), torch.zeros_like(r2))
     level = 0.5 * torch.log2(torch.clamp_min(major2, 1e-30))
     if mip_level_bias is not None:
         level = level + mip_level_bias
@@ -216,7 +221,9 @@ def texture(tex, uv, uv_da=None, mip_level_bias=None, mip=None, filter_mode="aut
     lod = _mip_level(uv_da.float(), tex.shape[1], tex.shape[2], len(levels), mip_level_bias)
     out = None
     for l, t in enumerate(levels):
-        w = torch.clamp(1.0 - (lod - float(l)).abs(), min=0.0)
+        # relu, not clamp: a level whose weight is exactly 0 (the neighbours of an integer LOD) also gets no gradient,
+        # so the result does not depend on whether that level is evaluated below
+        w = torch.relu(1.0 - (lod - float(l)).abs())
         if not bool((w > 0).any()):          # no pixel of this call uses the level
             continue
         term = w[..., None] * _Texture.apply(t, uv, bmode)

@@ -18,12 +18,17 @@ rast_db = (du/dX, du/dY, dv/dX, dv/dY) in pixel units; empty pixels are all zero
 
 Arithmetic contract (what makes triangle ids bit-exact against the CUDA path): coverage and depth are
 decided with 2-D homogeneous edge functions (no clipping needed) in IEEE fp32, no FMA, operation order as
-written in `_tri_setup` / `_edge_eval`; ties on shared edges are broken by a top-left rule on the edge
-coefficients; the depth test keeps the smallest z/w, ties -> smallest triangle index.
+written in `_tri_setup`, except that coverage takes the EXACT sign of each edge function (the fp32 value where it is
+outside its rounding error, rational arithmetic inside it), with exact zeros broken by a top-left rule on the exact
+edge coefficients (a symbolic perturbation: shared edges and vertices of closed fans on pixel centres are covered
+exactly once); u, v are fp64 edge-value quotients rounded once; the depth test keeps the smallest z/w,
+ties -> smallest triangle index.
 Gradients: to pos through u,v only (z/w, id and rast_db are treated as constants, which is all the
 reference's call sites need — `texture(filter_mode='linear')` ignores uv_da), to attr, tex, uv, color.
 """
 from __future__ import annotations
+
+from fractions import Fraction
 
 import numpy as np
 import torch
@@ -58,41 +63,106 @@ def _ordered_bits(zw: torch.Tensor) -> torch.Tensor:
     return k ^ 0x80000000          # top bit flipped so that (key << 32) orders correctly as a SIGNED int64
 
 
-def rasterize_ids(pos: torch.Tensor, tri: torch.Tensor, resolution, chunk=512):
-    """Integer part: winning triangle id+1 per pixel [B,h,w] (int64) — the bit-exact contract."""
+# Exact coverage signs.  Coverage is sign(e_i) * sign(det) > 0 with e_i = det[[x_j, x_k, X], [y_j, y_k, Y], [w_j, w_k, 1]].
+# The fp32 values decide when they are farther from 0 than their rounding error (gamma_5 times the sum of |terms|, over
+# |X|, |Y| <= 1, evaluated with slack: ERR_SCALE = 2^-20 ~ 16 u); otherwise the sign is computed exactly.  An exact 0 is
+# decided by the signs of the edge's (a, b) coefficients, taken exactly: the point is moved by (eps, eps^2), a
+# consistent symbolic perturbation under which a closed fan or a shared edge covers every point exactly once.  (The
+# kernels use the same fp32 filter, then fp64, then an exact expansion; any valid filter gives the same exact signs.)
+ERR_SCALE = 2.0 ** -20
+ERR_ABS = 1.0e-37
+
+
+def _edge_err(pj, pk):
+    f = torch.abs
+    return ((f(pj[..., 1] * pk[..., 3]) + f(pk[..., 1] * pj[..., 3])) + (f(pk[..., 0] * pj[..., 3]) + f(pj[..., 0] * pk[..., 3])) +
+            (f(pj[..., 0] * pk[..., 1]) + f(pk[..., 0] * pj[..., 1]))) * ERR_SCALE + ERR_ABS
+
+
+def _det_err(p0, p1, p2):
+    f = torch.abs
+    x0, y0, w0, x1, y1, w1, x2, y2, w2 = (p[..., k] for p in (p0, p1, p2) for k in (0, 1, 3))
+    return (f(x0) * (f(y1 * w2) + f(y2 * w1)) + f(x1) * (f(y2 * w0) + f(y0 * w2)) + f(x2) * (f(y0 * w1) + f(y1 * w0))) * ERR_SCALE + ERR_ABS
+
+
+def det3_sign_exact(c0, c1, c2) -> int:
+    """Sign of det[[x0, x1, x2], [y0, y1, y2], [w0, w1, w2]] for columns c_k = (x_k, y_k, w_k), in rational arithmetic."""
+    (x0, y0, w0), (x1, y1, w1), (x2, y2, w2) = [[Fraction(float(v)) for v in c] for c in (c0, c1, c2)]
+    d = x0 * (y1 * w2 - y2 * w1) - x1 * (y0 * w2 - y2 * w0) + x2 * (y0 * w1 - y1 * w0)
+    return (d > 0) - (d < 0)
+
+
+def edge_inside_exact(pj, pk, X, Y, sgn) -> bool:
+    """Exact coverage decision for the edge j -> k at the fp32 point (X, Y) of a triangle with orientation sgn (+-1)."""
+    s = det3_sign_exact((pj[0], pj[1], pj[3]), (pk[0], pk[1], pk[3]), (X, Y, 1.0)) * sgn
+    if s != 0:
+        return s > 0
+    F = lambda v: Fraction(float(v))
+    a_s = (F(pj[1]) * F(pk[3]) - F(pk[1]) * F(pj[3])) * sgn
+    b_s = (F(pk[0]) * F(pj[3]) - F(pj[0]) * F(pk[3])) * sgn
+    return a_s > 0 or (a_s == 0 and b_s > 0)
+
+
+def rasterize_ids(pos: torch.Tensor, tri: torch.Tensor, resolution, chunk=512, window=None):
+    """Integer part: winning triangle id+1 per pixel [B,h,w] (int64) — the bit-exact contract.
+    window=(y0, y1, x0, x1) evaluates only those pixels of the full frame (triangles whose bounding box misses the
+    window are culled first), which makes config-4-sized frames checkable piece by piece."""
     h, w = resolution
     B = pos.shape[0]
     pos = pos.detach().to(torch.float32)
     xs, ys = _pixel_ndc(h, w, torch.float32)
+    wy0, wy1, wx0, wx1 = window if window is not None else (0, h, 0, w)
+    xs, ys = xs[wx0:wx1], ys[wy0:wy1]
     X = xs[None, None, :]; Y = ys[None, :, None]
-    out = torch.zeros(B, h, w, dtype=torch.int64)
+    out = torch.zeros(B, wy1 - wy0, wx1 - wx0, dtype=torch.int64)
     tri = tri.to(torch.int64)
     F = tri.shape[0]
     BIG = torch.tensor(0x7FFFFFFFFFFFFFFF, dtype=torch.int64)
     for b in range(B):
-        best = torch.full((h, w), int(BIG), dtype=torch.int64)
-        for s in range(0, F, chunk):
-            t = tri[s:s + chunk]
+        best = torch.full((wy1 - wy0, wx1 - wx0), int(BIG), dtype=torch.int64)
+        fidx = torch.arange(F)
+        if window is not None and F > 0:
+            P = pos[b].double()[tri]                                             # [F,3,4]
+            front = (P[..., 3] > 0).all(dim=1)
+            Wc = torch.where(P[..., 3] > 0, P[..., 3], torch.ones_like(P[..., 3]))
+            sx_ = (P[..., 0] / Wc + 1.0) * (0.5 * w) - 0.5; sy_ = (P[..., 1] / Wc + 1.0) * (0.5 * h) - 0.5
+            keep = ~front | ((sx_.max(1).values >= wx0 - 2) & (sx_.min(1).values <= wx1 + 1) &
+                             (sy_.max(1).values >= wy0 - 2) & (sy_.min(1).values <= wy1 + 1))
+            fidx = fidx[keep]
+        for s in range(0, fidx.numel(), chunk):
+            ids_c = fidx[s:s + chunk]
+            t = tri[ids_c]
             p0, p1, p2 = pos[b, t[:, 0]], pos[b, t[:, 1]], pos[b, t[:, 2]]
             (a0, b0, c0), (a1, b1, c1), (a2, b2, c2), det = _tri_setup(p0, p1, p2)
             sgn = torch.where(det < 0, -torch.ones_like(det), torch.ones_like(det))
             ok = det != 0
+            unsure_det = torch.nonzero(ok & (det.abs() <= _det_err(p0, p1, p2)), as_tuple=True)[0]
+            for k in unsure_det.tolist():
+                sg = det3_sign_exact(*[(q[k, 0].item(), q[k, 1].item(), q[k, 3].item()) for q in (p0, p1, p2)])
+                sgn[k] = float(sg) if sg != 0 else 1.0
+                ok[k] = sg != 0
 
             def ev(a, bb, c):
                 return (a[:, None, None] * X + bb[:, None, None] * Y) + c[:, None, None]
-
-            def inside(e, a, bb):
-                es = e * sgn[:, None, None]
-                a_s = (a * sgn)[:, None, None]; b_s = (bb * sgn)[:, None, None]
-                return (es > 0) | ((es == 0) & ((a_s > 0) | ((a_s == 0) & (b_s > 0))))
             e0, e1, e2 = ev(a0, b0, c0), ev(a1, b1, c1), ev(a2, b2, c2)
-            cov = inside(e0, a0, b0) & inside(e1, a1, b1) & inside(e2, a2, b2) & ok[:, None, None]
+            sg3 = sgn[:, None, None]
+            verts = (p0, p1, p2)
+            ins, unsure = [], []
+            for i, e in enumerate((e0, e1, e2)):
+                sure = e.abs() > _edge_err(verts[(i + 1) % 3], verts[(i + 2) % 3])[:, None, None]
+                ins.append(sure & (e * sg3 > 0)); unsure.append(~sure)
+            cov = (ins[0] | unsure[0]) & (ins[1] | unsure[1]) & (ins[2] | unsure[2]) & ok[:, None, None]
+            for i in range(3):                                       # settle the edges inside their rounding band
+                ff, yy, xx = torch.nonzero(cov & unsure[i], as_tuple=True)
+                pj, pk = verts[(i + 1) % 3], verts[(i + 2) % 3]
+                for f_, y_, x_ in zip(ff.tolist(), yy.tolist(), xx.tolist()):
+                    if not edge_inside_exact(pj[f_].tolist(), pk[f_].tolist(), xs[x_].item(), ys[y_].item(), sgn[f_].item()):
+                        cov[f_, y_, x_] = False
             z0, z1, z2 = p0[:, 2], p1[:, 2], p2[:, 2]
             dets = torch.where(ok, det, torch.ones_like(det))
             zw = ((z0[:, None, None] * e0 + z1[:, None, None] * e1) + z2[:, None, None] * e2) / dets[:, None, None]
             cov = cov & (zw >= -1.0) & (zw <= 1.0)
-            ids = torch.arange(s, s + t.shape[0], dtype=torch.int64)[:, None, None]
-            key = (_ordered_bits(zw) << 32) | ids
+            key = (_ordered_bits(zw) << 32) | ids_c[:, None, None]
             key = torch.where(cov, key, BIG)
             best = torch.minimum(best, key.min(dim=0).values)
         hit = best != BIG
@@ -106,7 +176,8 @@ def rasterize(pos: torch.Tensor, tri: torch.Tensor, resolution):
     B = pos.shape[0]
     dt = pos.dtype
     ids = rasterize_ids(pos, tri, resolution)                        # [B,h,w]
-    xs, ys = _pixel_ndc(h, w, dt)
+    xs, ys = _pixel_ndc(h, w, torch.float32)                         # the fp32 pixel centres the kernels use, exactly
+    xs, ys = xs.to(dt), ys.to(dt)
     X = xs[None, None, :].expand(B, h, w); Y = ys[None, :, None].expand(B, h, w)
     hit = ids > 0
     t = tri.to(torch.int64)[(ids - 1).clamp_min(0)]                  # [B,h,w,3]
@@ -117,7 +188,15 @@ def rasterize(pos: torch.Tensor, tri: torch.Tensor, resolution):
     S = e0 + e1 + e2
     S = torch.where(hit, S, torch.ones_like(S))
     dets = torch.where(hit, det, torch.ones_like(det))
-    u = e0 / S; v = e1 / S
+    # coverage is exact, so at a pixel within rounding of an edge e_i may have the sign opposite to the triangle's: it
+    # is then replaced by 0 (closer to the exact value), so that u, v, 1 - u - v >= 0
+    sg = torch.where(S < 0, -torch.ones_like(S), torch.ones_like(S))
+    c0, c1, c2 = (torch.where(e * sg < 0, torch.zeros_like(e), e) for e in (e0, e1, e2))
+    Sc = c0 + c1 + c2
+    okc = Sc != 0
+    Scs = torch.where(okc, Sc, torch.ones_like(Sc))
+    u0, v0 = e0 / S, e1 / S                            # the gradient is that of the unclamped values, as in the kernel
+    u = u0 + (torch.where(okc, c0 / Scs, u0) - u0).detach(); v = v0 + (torch.where(okc, c1 / Scs, v0) - v0).detach()
     zw = (((p0[..., 2] * e0 + p1[..., 2] * e1) + p2[..., 2] * e2) / dets).detach()
     sa, sb = a0 + a1 + a2, b0 + b1 + b2
     sx, sy = 2.0 / w, 2.0 / h
@@ -177,7 +256,12 @@ def mip_level(uv_da: torch.Tensor, Ht: int, Wt: int, n_levels: int, mip_level_bi
     A = dsdx * dsdx + dtdx * dtdx
     Bq = dsdy * dsdy + dtdy * dtdy
     Cq = dsdx * dsdy + dtdx * dtdy
-    major2 = 0.5 * (A + Bq) + torch.sqrt(0.25 * (A - Bq) * (A - Bq) + Cq * Cq)
+    r2 = 0.25 * (A - Bq) * (A - Bq) + Cq * Cq
+    # sqrt guarded at 0 (every isotropic footprint, and uv_da = 0): same value, and the root's subgradient 0 there instead
+    # of sqrt's infinite derivative (which made d uv_da NaN); along any direction the gradient is then the mean of the
+    # two one-sided derivatives
+    pos_r2 = r2 > 0
+    major2 = 0.5 * (A + Bq) + torch.where(pos_r2, torch.sqrt(torch.where(pos_r2, r2, torch.ones_like(r2))), torch.zeros_like(r2))
     level = 0.5 * torch.log2(torch.clamp_min(major2, 1e-30))
     if mip_level_bias is not None:
         level = level + mip_level_bias
@@ -194,7 +278,7 @@ def texture(tex: torch.Tensor, uv: torch.Tensor, filter_mode="linear", boundary_
         lod = mip_level(uv_da, tex.shape[1], tex.shape[2], len(levels), mip_level_bias)
         out = 0
         for l, t in enumerate(levels):
-            w = torch.clamp(1.0 - (lod - float(l)).abs(), min=0.0)              # tent weight = the two-level lerp
+            w = torch.relu(1.0 - (lod - float(l)).abs())              # tent weight = the two-level lerp
             out = out + w[..., None] * texture(t, uv, "linear", boundary_mode)
         return out
     assert filter_mode == "linear"
@@ -368,3 +452,67 @@ def clip_positions(v: torch.Tensor, pose: np.ndarray, proj: np.ndarray) -> torch
     pose = torch.from_numpy(pose.astype(np.float32)); proj = torch.from_numpy(proj.astype(np.float32))
     v_cam = torch.matmul(torch.nn.functional.pad(v, pad=(0, 1), mode="constant", value=1.0), torch.inverse(pose).T).float().unsqueeze(0)
     return v_cam @ proj.T
+
+
+def pixel_centre(i: int, n: int) -> float:
+    """The fp32 NDC coordinate of pixel centre i of n, as the rasterizer computes it: (i + 0.5) * fl(2/n) - 1."""
+    return float(np.float32(np.float32(i + 0.5) * np.float32(2.0 / n) - np.float32(1.0)))
+
+
+def pixel_centre_fan(rng, H, W, perspective, k=None):
+    """A closed fan of k (5..9) triangles around a centre vertex exactly on a pixel centre (a power-of-two w keeps x/w
+    exact); ring radius 4..9 px, angular gaps below 2 rad, ring w in [0.5, 3] when perspective.
+    Returns (pos [1,k+1,4] f32, tri [k,3] i32, (px, py))."""
+    k = int(rng.integers(5, 10)) if k is None else k
+    while True:
+        ang = np.sort(rng.uniform(0, 2 * np.pi, k))
+        if np.max(np.diff(np.concatenate([ang, [ang[0] + 2 * np.pi]]))) < 2.0:
+            break
+    px, py = int(rng.integers(10, W - 10)), int(rng.integers(10, H - 10))
+    cx, cy = pixel_centre(px, W), pixel_centre(py, H)
+    wc = float(2.0 ** rng.integers(-1, 2)) if perspective else 1.0
+    r = rng.uniform(4.0, 9.0, k)
+    wr = rng.uniform(0.5, 3.0, k) if perspective else np.ones(k)
+    rows = [[cx * wc, cy * wc, 0.0, wc]]
+    for i in range(k):
+        x = cx + r[i] * np.cos(ang[i]) * 2.0 / W; y = cy + r[i] * np.sin(ang[i]) * 2.0 / H
+        rows.append([x * wr[i], y * wr[i], 0.25 * wr[i], wr[i]])
+    tri = [[0, 1 + i, 1 + (i + 1) % k] if i % 2 == 0 else [0, 1 + (i + 1) % k, 1 + i] for i in range(k)]   # mixed winding
+    return torch.tensor([rows], dtype=torch.float32), torch.tensor(tri, dtype=torch.int32), (px, py)
+
+
+def pixel_centre_grid(H, W, step, x0, y0, nx, ny, z=0.0):
+    """UV-bake style grid (w = 1) whose (nx+1) x (ny+1) vertices lie exactly on the fp32 centres of pixels
+    (x0 + i step, y0 + j step); cells split along alternating diagonals.  Returns (pos [1,V,4] f32, tri [F,3] i32)."""
+    xs = [pixel_centre(x0 + i * step, W) for i in range(nx + 1)]
+    ys = [pixel_centre(y0 + j * step, H) for j in range(ny + 1)]
+    pos = torch.tensor([[[x, y, z, 1.0] for y in ys for x in xs]], dtype=torch.float32)
+    tri = []
+    for j in range(ny):
+        for i in range(nx):
+            a = j * (nx + 1) + i; b = a + 1; c = a + nx + 1; d = c + 1
+            tri += [[a, b, d], [a, d, c]] if (i + j) % 2 == 0 else [[a, b, c], [b, d, c]]
+    return pos, torch.tensor(tri, dtype=torch.int32)
+
+
+def coverage_count(pos: torch.Tensor, tri: torch.Tensor, resolution):
+    """[B,h,w] number of triangles covering each pixel centre, each triangle rasterized on its own (over the window of
+    its bounding box)."""
+    h, w = resolution
+    B = pos.shape[0]
+    cnt = torch.zeros(B, h, w, dtype=torch.int64)
+    P = pos.detach().double()
+    for f in range(tri.shape[0]):
+        t = tri[f:f + 1]
+        q = P[:, t[0].long()]                                                        # [B,3,4]
+        if bool((q[..., 3] > 0).all()):
+            sx = (q[..., 0] / q[..., 3] + 1.0) * (0.5 * w) - 0.5; sy = (q[..., 1] / q[..., 3] + 1.0) * (0.5 * h) - 0.5
+            win = (max(0, int(np.floor(float(sy.min()))) - 2), min(h, int(np.ceil(float(sy.max()))) + 3),
+                   max(0, int(np.floor(float(sx.min()))) - 2), min(w, int(np.ceil(float(sx.max()))) + 3))
+            if win[0] >= win[1] or win[2] >= win[3]:
+                continue
+        else:
+            win = (0, h, 0, w)
+        ids = rasterize_ids(pos, t, resolution, window=win)
+        cnt[:, win[0]:win[1], win[2]:win[3]] += (ids > 0).to(torch.int64)
+    return cnt

@@ -180,3 +180,87 @@ def test_mipmapped_texture_levels_and_limits():
         got = D.texture(tex, uv, "linear-mipmap-linear", uv_da=da)
         assert torch.allclose(got, D.texture(pyr[k], uv, "linear"), atol=1e-6), k
     assert float(D.mip_level(torch.full((1, 1, 1, 4), 100.0), 16, 32, len(pyr)).max()) == len(pyr) - 1      # clamped
+
+
+# ---------------- scenes with vertices and edges exactly on pixel centres; the windowed evaluation ----------------------
+def test_fan_premise_centre_vertex_is_on_the_fp32_pixel_centre():
+    from fractions import Fraction
+    rng = np.random.default_rng(1)
+    for persp in (False, True):
+        pos, tri, (px, py) = D.pixel_centre_fan(rng, 64, 64, persp)
+        x, y, _, w = pos[0, 0].tolist()
+        assert Fraction(x) / Fraction(w) == Fraction(D.pixel_centre(px, 64))
+        assert Fraction(y) / Fraction(w) == Fraction(D.pixel_centre(py, 64))
+        assert len({tuple(sorted(t)) for t in tri.tolist()}) == tri.shape[0]
+
+
+@pytest.mark.parametrize("persp", [False, True])
+def test_closed_fans_around_pixel_centre_vertices_cover_every_pixel_once(persp):
+    """At a vertex exactly on a pixel centre each spoke's fp32 edge value is rounding noise of either sign; with the
+    fp32 signs alone 8 of 253 random fans left the centre pixel uncovered (a hole in a closed surface) and 134 covered
+    it twice.  Exact signs with the symbolic tie rule cover every pixel of every fan exactly once."""
+    rng = np.random.default_rng(123 + persp)
+    for _ in range(75):
+        pos, tri, (px, py) = D.pixel_centre_fan(rng, 64, 64, persp)
+        cnt = D.coverage_count(pos, tri, (64, 64))[0]
+        assert int(cnt.max()) == 1, (px, py)
+        assert bool((cnt[py - 1:py + 2, px - 1:px + 2] == 1).all()), (px, py)      # inside the ring (inradius > 2 px)
+
+
+def test_pixel_centre_grid_is_watertight():
+    """A grid whose vertices all lie on pixel centres (a UV-space bake): every pixel strictly inside it, vertex pixels
+    included, is covered exactly once."""
+    H = W = 64
+    pos, tri = D.pixel_centre_grid(H, W, 3, 5, 4, 17, 18)
+    cnt = D.coverage_count(pos, tri, (H, W))[0]
+    assert int(cnt.max()) == 1
+    assert bool((cnt[5:58, 6:56] == 1).all())
+    ids = D.rasterize_ids(pos, tri, (H, W))[0]
+    assert bool(((ids > 0) == (cnt > 0)).all())
+
+
+def test_exact_sign_helpers():
+    c = D.pixel_centre(20, 64)
+    assert D.det3_sign_exact((0.0, 0.0, 1.0), (1.0, 0.0, 1.0), (0.0, 1.0, 1.0)) == 1
+    assert D.det3_sign_exact((0.0, 1.0, 1.0), (1.0, 0.0, 1.0), (0.0, 0.0, 1.0)) == -1
+    assert D.det3_sign_exact((c, c, 1.0), (2 * c, 2 * c, 2.0), (0.3, 0.1, 1.0)) == 0       # same point projectively
+    # an edge through the point: exact zero, decided by (a, b): exactly one of the two orientations covers it
+    pj, pk = [c, -0.5, 0.0, 1.0], [c, 0.5, 0.0, 1.0]
+    assert D.edge_inside_exact(pj, pk, c, 0.0, 1.0) != D.edge_inside_exact(pk, pj, c, 0.0, 1.0)
+
+
+def test_window_mode_matches_the_full_frame():
+    v, f, _ = D.icosphere(2)
+    pos = D.clip_positions(v, O.orbit_camera(20, 30, 1.75), D.gl_perspective(49.1, 1.0))
+    full = D.rasterize_ids(pos, f, (48, 48))
+    assert torch.equal(D.rasterize_ids(pos, f, (48, 48), window=(10, 30, 5, 41)), full[:, 10:30, 5:41])
+
+
+# ---------------- mip level: finite gradient at isotropic and zero footprints ---------------------------------------
+@pytest.mark.parametrize("da", [(0.01, 0.0, 0.0, 0.01), (0.0, 0.0, 0.0, 0.0), (0.01, 0.002, 0.0, 0.01), (0.004, 0.0, 0.0, 0.0)])
+def test_mip_level_gradient_is_finite(da):
+    x = torch.tensor(da, dtype=torch.float64).reshape(1, 1, 1, 4).requires_grad_(True)
+    D.mip_level(x, 64, 64, 7).sum().backward()
+    assert bool(torch.isfinite(x.grad).all())
+
+
+def test_mip_level_subgradient_at_the_isotropic_point():
+    """At an isotropic footprint (A = B, C = 0) the root term sqrt(0.25 (A-B)^2 + C^2) is a cone point; its gradient is
+    taken as 0 there, so the level's gradient is the mean of the two one-sided derivatives along every direction, and
+    the derivative itself along directions that keep the footprint isotropic (scaling and rotating uv_da)."""
+    x0 = torch.tensor([0.05, 0.0, 0.0, 0.05], dtype=torch.float64)
+    f = lambda x: float(D.mip_level(x.reshape(1, 1, 1, 4), 64, 64, 7).sum())
+    x = x0.clone().reshape(1, 1, 1, 4).requires_grad_(True)
+    D.mip_level(x, 64, 64, 7).sum().backward()
+    g = x.grad.reshape(4)
+    assert bool(torch.isfinite(g).all()) and float(g.abs().max()) > 0
+    h = 1e-7
+    for d in (x0, torch.tensor([0.0, 0.05, -0.05, 0.0], dtype=torch.float64)):            # scale; rotate
+        right = (f(x0 + h * d) - f(x0)) / h
+        assert abs(right - float(g @ d)) <= 1e-6 * max(1.0, abs(right))
+    rng = np.random.default_rng(0)
+    for _ in range(5):
+        d = torch.from_numpy(rng.standard_normal(4))
+        right = (f(x0 + h * d) - f(x0)) / h; left = (f(x0) - f(x0 - h * d)) / h
+        assert left - 1e-6 <= float(g @ d) <= right + 1e-6
+        assert abs(0.5 * (left + right) - float(g @ d)) <= 1e-5 * max(1.0, abs(right))
