@@ -82,6 +82,31 @@ int32_t ngp_b200_mcubes_count(const float* volume, int32_t X, int32_t Y, int32_t
 int32_t ngp_b200_mcubes_write(const float* volume, int32_t X, int32_t Y, int32_t Z, float iso,
                               const unsigned long long* totals_host3, float* verts, int32_t* tris, void* scratch,
                               void* stream);
+/* ---- FlexiCubes triangle-mesh extraction (FlexiCubes.__call__, MVs_Algorithms/FlexiCubes/flexicubes.py) on the
+ * regular grid of Rx x Ry x Rz cubes: point (i,j,k) = (i*(Ry+1) + j)*(Rz+1) + k, x[P,3] and s[P] fp32 contiguous.
+ * Raw weights beta[F,12], alpha[F,8], gamma[F] are fp32 rows with the given row strides (unit column stride), or NULL
+ * for all ones; cube (i,j,k) = (i*Ry + j)*Rz + k.  count -> (host copies totals_dev4) -> write.  totals = {dual
+ * vertices, L_dev entries, quads, surface cubes}.  write: verts[V,3] (V = vertices + training * quads), faces[T,3]
+ * int64 (T = 2 or 4 per quad), L_dev[E].  backward needs no host read: grad_verts[V,3] and grad_ldev[E] in, and any
+ * of grad_x[P,3], grad_s[P], grad_beta[F,12], grad_alpha[F,8], grad_gamma[F] (dense, contiguous; NULL = not wanted)
+ * written in full, from a fixed summation order (bit-identical from run to run).  scratch >= flexicubes_scratch_bytes
+ * is passed unchanged from count to write to backward; workspace >= flexicubes_backward_workspace_bytes. */
+size_t ngp_b200_flexicubes_scratch_bytes(int32_t Rx, int32_t Ry, int32_t Rz);
+int32_t ngp_b200_flexicubes_count(const float* s, int32_t Rx, int32_t Ry, int32_t Rz,
+                                  unsigned long long* totals_dev4, void* scratch, void* stream);
+int32_t ngp_b200_flexicubes_write(const float* x, const float* s, const float* beta, int64_t beta_stride,
+                                  const float* alpha, int64_t alpha_stride, const float* gamma, int64_t gamma_stride,
+                                  int32_t Rx, int32_t Ry, int32_t Rz, double weight_scale, int32_t training,
+                                  const unsigned long long* totals_host4, float* verts, int64_t* faces, float* ldev,
+                                  void* scratch, void* stream);
+size_t ngp_b200_flexicubes_backward_workspace_bytes(const unsigned long long* totals_host4, int32_t training);
+int32_t ngp_b200_flexicubes_backward(const float* x, const float* s, const float* beta, int64_t beta_stride,
+                                     const float* alpha, int64_t alpha_stride, const float* gamma,
+                                     int64_t gamma_stride, int32_t Rx, int32_t Ry, int32_t Rz, double weight_scale,
+                                     int32_t training, const unsigned long long* totals_host4, const float* verts,
+                                     const float* grad_verts, const float* grad_ldev, float* grad_x, float* grad_s,
+                                     float* grad_beta, float* grad_alpha, float* grad_gamma, void* scratch,
+                                     void* workspace, void* stream);
 #ifdef __cplusplus
 }
 #endif
