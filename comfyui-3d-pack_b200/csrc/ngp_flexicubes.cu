@@ -7,6 +7,13 @@
 // per-point pass that gathers the corner partials of its 8 cubes in a fixed order.  No fp32 atomics anywhere, so
 // gradients are bit-identical from run to run.
 //
+// Attributes (the TRELLIS / Stable3DGen variant, ngp_b200_flexicubes_*_attrs): C channels per grid point, activated by
+// a sigmoid, crossed on each group edge with the same end weights s * alpha as the dual vertex and averaged with the
+// same beta; training quad centres take the same gamma-weighted diagonal means.  They are the `ATTRS` instantiation of the
+// same passes; the C = 0 instantiation is the attribute-free extraction, unchanged.  Their backward adds their terms
+// after the geometry's, writes per-corner attribute partials next to the geometry's, and the per-point pass gathers
+// them in the same corner order.
+//
 // Numbering: point (i,j,k) = (i*Sy + j)*Sz + k, cube (i,j,k) = (i*Ry + j)*Rz + k, S = R + 1; corner c of a cube is
 // the point at offset (c&1, (c>>1)&1, c>>2); case bit c = s < 0.  Output order: dual vertices by (cube, group),
 // then (training) one centre per quad; quads by (owning cube, axis), the owner being the lowest of the 4 cubes, whose
@@ -34,6 +41,11 @@ struct FcWeights {
     const float* alpha; long long sa;
     const float* gamma; long long sg;
     float ws, ws_half;                  // weight_scale, (1 - weight_scale) / 2
+};
+
+struct FcAttrs {
+    const float* a; long long stride;   // raw attributes, row stride (unit column stride); NULL when C = 0
+    int C;
 };
 
 // axis of each cube edge, and the order of the 4 cubes around an owned edge: cube offset (along the two other axes,
@@ -83,6 +95,7 @@ __device__ __forceinline__ uint32_t owned_quads(const FcGrid& g, uint32_t c, int
 __device__ __forceinline__ float tanh_w(const float* w, long long stride, long long f, int c, float ws) {
     return w ? __fadd_rn(__fmul_rn(tanhf(__ldg(w + f * stride + c)), ws), 1.f) : 1.f;
 }
+__device__ __forceinline__ float sigmoid_f(float r) { return 1.f / (1.f + expf(-r)); }
 __device__ __forceinline__ float gamma_w(const FcWeights& W, long long f) {
     if (!W.gamma) return 1.f;
     const float sg = 1.f / (1.f + expf(-__ldg(W.gamma + f * W.sg)));
@@ -166,12 +179,23 @@ __device__ __forceinline__ int dual_vertex(const FcGrid& g, const float* __restr
     return n;
 }
 
+// attribute ch crossed on group edge E with the end weights (wa, wb) of its ue: (ca wb - cb wa) / (wb - wa)
+__device__ __forceinline__ float attr_crossing(const FcGrid& g, const FcAttrs& A, long long p0, const EdgeEval& E,
+                                               int ch, float& ca, float& cb) {
+    ca = sigmoid_f(__ldg(A.a + corner_point(g, p0, E.ca) * A.stride + ch));
+    cb = sigmoid_f(__ldg(A.a + corner_point(g, p0, E.cb) * A.stride + ch));
+    const float wa = E.sa * E.aa, wb = E.sb * E.ab;
+    return (ca * wb - cb * wa) / (wb - wa);
+}
+
+template <bool ATTRS>
 __global__ void __launch_bounds__(FC_THREADS) fc_vertex_kernel(const float* __restrict__ x, const float* __restrict__ s,
-                                                               const FcGrid g, const FcWeights W,
+                                                               const FcGrid g, const FcWeights W, const FcAttrs A,
                                                                const uint8_t* __restrict__ cases,
                                                                const uint32_t* __restrict__ voff,
                                                                const uint32_t* __restrict__ loff,
-                                                               float* __restrict__ verts, float* __restrict__ ldev) {
+                                                               float* __restrict__ verts, float* __restrict__ ldev,
+                                                               float* __restrict__ vattrs) {
     const long long f = blockIdx.x * (long long)FC_THREADS + threadIdx.x;
     if (f >= g.F) return;
     const uint32_t c = cases[f];
@@ -196,6 +220,13 @@ __global__ void __launch_bounds__(FC_THREADS) fc_vertex_kernel(const float* __re
         }
         mean /= (float)n;
         for (int t = 0; t < n; t++) ldev[l++] = fabsf(dist[t] - mean);
+        if constexpr (ATTRS) {
+            for (int ch = 0; ch < A.C; ch++) {
+                float acc = 0.f, ca, cb;
+                for (int t = 0; t < n; t++) acc += beta[t] * attr_crossing(g, A, p0, E[t], ch, ca, cb);
+                vattrs[(long long)v * A.C + ch] = acc / bsum;
+            }
+        }
     }
 }
 
@@ -225,12 +256,14 @@ __device__ __forceinline__ void owned_quad(const FcGrid& g, const float* __restr
     for (int t = 0; t < 4; t++) Q.order[t] = flip ? o1[t] : o2[t];
 }
 
+template <bool ATTRS>
 __global__ void __launch_bounds__(FC_THREADS) fc_quad_kernel(const float* __restrict__ s, const FcGrid g,
                                                              const FcWeights W, const uint8_t* __restrict__ cases,
                                                              const uint32_t* __restrict__ voff,
                                                              const uint32_t* __restrict__ qoff, uint32_t nvd,
                                                              int training, float* __restrict__ verts,
-                                                             int64_t* __restrict__ faces) {
+                                                             int64_t* __restrict__ faces, int C,
+                                                             float* __restrict__ vattrs) {
     const long long f = blockIdx.x * (long long)FC_THREADS + threadIdx.x;
     if (f >= g.F) return;
     const uint32_t c = cases[f];
@@ -260,6 +293,13 @@ __global__ void __launch_bounds__(FC_THREADS) fc_quad_kernel(const float* __rest
                 const float a13 = (verts[3 * v[1] + d] + verts[3 * v[3] + d]) / 2.f;
                 verts[3 * ctr + d] = (a02 * g02 + a13 * g13) / wsum;
             }
+            if constexpr (ATTRS) {
+                for (int ch = 0; ch < C; ch++) {
+                    const float a02 = (vattrs[v[0] * C + ch] + vattrs[v[2] * C + ch]) / 2.f;
+                    const float a13 = (vattrs[v[1] * C + ch] + vattrs[v[3] * C + ch]) / 2.f;
+                    vattrs[ctr * C + ch] = (a02 * g02 + a13 * g13) / wsum;
+                }
+            }
             int64_t* o = faces + 12ll * q;
 #pragma unroll
             for (int t = 0; t < 4; t++) { o[3 * t] = v[t]; o[3 * t + 1] = v[(t + 1) & 3]; o[3 * t + 2] = ctr; }
@@ -270,14 +310,19 @@ __global__ void __launch_bounds__(FC_THREADS) fc_quad_kernel(const float* __rest
 
 // ---- backward ---------------------------------------------------------------------------------------------------
 
-// per quad slot (cube ascending): d loss / d (its dual vertex) in xyz, d loss / d (its cube's normalised gamma) in w
+// per quad slot (cube ascending): d loss / d (its dual vertex) in xyz, d loss / d (its cube's normalised gamma) in w;
+// with attributes, w also takes their terms and qh holds d centre / d (the slot's dual vertex), the same per channel
+template <bool ATTRS>
 __global__ void __launch_bounds__(FC_THREADS) fc_quad_bwd_kernel(const float* __restrict__ s, const FcGrid g,
                                                                  const FcWeights W, const uint8_t* __restrict__ cases,
                                                                  const uint32_t* __restrict__ voff,
                                                                  const uint32_t* __restrict__ qoff, uint32_t nvd,
                                                                  const float* __restrict__ verts,
                                                                  const float* __restrict__ gverts,
-                                                                 float4* __restrict__ qpart) {
+                                                                 float4* __restrict__ qpart, int C,
+                                                                 const float* __restrict__ vattrs,
+                                                                 const float* __restrict__ gvattrs,
+                                                                 float* __restrict__ qh) {
     const long long f = blockIdx.x * (long long)FC_THREADS + threadIdx.x;
     if (f >= g.F) return;
     const uint32_t c = cases[f];
@@ -306,6 +351,17 @@ __global__ void __launch_bounds__(FC_THREADS) fc_quad_bwd_kernel(const float* __
             d02 += gc[d] * (a02 - ctr[d]);
             d13 += gc[d] * (a13 - ctr[d]);
         }
+        if constexpr (ATTRS) {
+            const uint64_t V[4] = {Q.v[Q.order[0]], Q.v[Q.order[1]], Q.v[Q.order[2]], Q.v[Q.order[3]]};
+            const uint64_t ci = (uint64_t)(nvd + q) * C;
+            for (int ch = 0; ch < C; ch++) {
+                const float a02 = (vattrs[V[0] * C + ch] + vattrs[V[2] * C + ch]) / 2.f;
+                const float a13 = (vattrs[V[1] * C + ch] + vattrs[V[3] * C + ch]) / 2.f;
+                const float ct = vattrs[ci + ch], gct = gvattrs[ci + ch];
+                d02 += gct * (a02 - ct);
+                d13 += gct * (a13 - ct);
+            }
+        }
         const float gg02 = d02 / wsum, gg13 = d13 / wsum;
         const float h02 = g02 / wsum / 2.f, h13 = g13 / wsum / 2.f;
         const float gg[4] = {gg02 * ga[2], gg13 * ga[3], gg02 * ga[0], gg13 * ga[1]};
@@ -313,6 +369,7 @@ __global__ void __launch_bounds__(FC_THREADS) fc_quad_bwd_kernel(const float* __
         for (int t = 0; t < 4; t++) {
             const float h = (t & 1) ? h13 : h02;
             qpart[4ull * q + Q.order[t]] = make_float4(gc[0] * h, gc[1] * h, gc[2] * h, gg[t]);
+            if constexpr (ATTRS) qh[4ull * q + Q.order[t]] = h;
         }
         q++;
     }
@@ -333,12 +390,47 @@ __device__ __forceinline__ void crossing_bwd(const float* xa, const float* xb, f
     gwb += db / den;
 }
 
+// the quad that cube (i,j,k)'s crossed edge e belongs to, and the cube's slot in it; false when the edge lies on the
+// grid's boundary (fewer than 4 cubes, no quad)
+__device__ __forceinline__ bool quad_slot(const FcGrid& g, const uint8_t* __restrict__ cases,
+                                          const uint32_t* __restrict__ qoff, int i, int j, int k, int e,
+                                          uint32_t& q, int& slot) {
+    const int ijk[3] = {i, j, k}, R[3] = {g.Rx, g.Ry, g.Rz};
+    const int a = fc_edge_axis[e], c0 = fc_cube_edges[e][0];
+    const int off[3] = {c0 & 1, (c0 >> 1) & 1, c0 >> 2};
+    int o[3] = {i, j, k};
+    bool interior = true;
+    for (int b = 0; b < 3; b++) {
+        if (b == a) continue;
+        const int gp = ijk[b] + off[b];
+        interior &= gp >= 1 && gp <= R[b] - 1;
+        o[b] = gp - 1;
+    }
+    if (!interior) return false;
+    const long long of = cube_id(g, o[0], o[1], o[2]);
+    const uint32_t om = owned_quads(g, cases[of], o[0], o[1], o[2]);
+    q = qoff[of] + __popc(om & ((1u << a) - 1u));
+    const int b1 = a == 0 ? 1 : 0, b2 = a == 2 ? 1 : 2;
+    slot = 2 * (1 - off[b1]) + (1 - off[b2]);
+    return true;
+}
+
+// attribute inputs of the cube backward: per-vertex output gradients, the quad-centre factors (training) and the
+// per-corner partials of the surface cubes (NULL when no attribute gradient is wanted)
+struct FcAttrGrads {
+    const float* gvattrs;
+    const float* qh;
+    float* cattr;
+};
+
+template <bool ATTRS>
 __global__ void __launch_bounds__(FC_THREADS) fc_cube_bwd_kernel(
     const float* __restrict__ x, const float* __restrict__ s, const FcGrid g, const FcWeights W,
     const uint8_t* __restrict__ cases, const uint32_t* __restrict__ voff, const uint32_t* __restrict__ loff,
     const uint32_t* __restrict__ qoff, const uint32_t* __restrict__ soff, const float* __restrict__ gverts,
     const float* __restrict__ gldev, const float4* __restrict__ qpart, float4* __restrict__ cpart,
-    float* __restrict__ gbeta, float* __restrict__ galpha, float* __restrict__ ggamma) {
+    float* __restrict__ gbeta, float* __restrict__ galpha, float* __restrict__ ggamma, const FcAttrs A,
+    const FcAttrGrads AG, uint32_t nvd) {
     const long long f = blockIdx.x * (long long)FC_THREADS + threadIdx.x;
     if (f >= g.F) return;
     const uint32_t c = cases[f];
@@ -350,8 +442,14 @@ __global__ void __launch_bounds__(FC_THREADS) fc_cube_bwd_kernel(
     if (is_surface(c)) {
         int i, j, k;
         cube_ijk(g, f, i, j, k);
-        const int ijk[3] = {i, j, k}, R[3] = {g.Rx, g.Ry, g.Rz};
         const long long p0 = point_id(g, i, j, k);
+        float* cattr = nullptr;
+        if constexpr (ATTRS) {
+            if (AG.cattr) {
+                cattr = AG.cattr + 8ull * soff[f] * A.C;
+                for (int t = 0; t < 8 * A.C; t++) cattr[t] = 0.f;
+            }
+        }
         uint32_t v = voff[f], l = loff[f];
         for (int gi = 0; gi < fc_num_vd[c]; gi++, v++) {
             EdgeEval E[FC_MAX_GROUP_EDGES];
@@ -361,22 +459,9 @@ __global__ void __launch_bounds__(FC_THREADS) fc_cube_bwd_kernel(
             // quad-centre partials of this dual vertex, in group edge order
             if (qpart) {
                 for (int t = 0; t < n; t++) {
-                    const int e = fc_groups[c][gi][t], a = fc_edge_axis[e], c0 = fc_cube_edges[e][0];
-                    const int off[3] = {c0 & 1, (c0 >> 1) & 1, c0 >> 2};
-                    int o[3] = {i, j, k};
-                    bool interior = true;
-                    for (int b = 0; b < 3; b++) {
-                        if (b == a) continue;
-                        const int gp = ijk[b] + off[b];
-                        interior &= gp >= 1 && gp <= R[b] - 1;
-                        o[b] = gp - 1;
-                    }
-                    if (!interior) continue;
-                    const long long of = cube_id(g, o[0], o[1], o[2]);
-                    const uint32_t om = owned_quads(g, cases[of], o[0], o[1], o[2]);
-                    const uint32_t q = qoff[of] + __popc(om & ((1u << a) - 1u));
-                    const int b1 = a == 0 ? 1 : 0, b2 = a == 2 ? 1 : 2;
-                    const int slot = 2 * (1 - off[b1]) + (1 - off[b2]);
+                    uint32_t q;
+                    int slot;
+                    if (!quad_slot(g, cases, qoff, i, j, k, fc_groups[c][gi][t], q, slot)) continue;
                     const float4 p = qpart[4ull * q + slot];
                     gvd[0] += p.x; gvd[1] += p.y; gvd[2] += p.z;
                     ggam += p.w;
@@ -432,6 +517,43 @@ __global__ void __launch_bounds__(FC_THREADS) fc_cube_bwd_kernel(
                 gan[E[t].ca] += gwa * E[t].sa;
                 gan[E[t].cb] += gwb * E[t].sb;
             }
+            // attributes, after the geometry: va = sum(beta uc) / sum(beta), uc the crossing of sigmoid(raw) with
+            // the end weights of ue; the vertex's gradient takes its quad-centre terms in group edge order
+            if constexpr (ATTRS) {
+                long long qslot[FC_MAX_GROUP_EDGES], qctr[FC_MAX_GROUP_EDGES];
+                for (int t = 0; t < n; t++) {
+                    uint32_t q;
+                    int slot;
+                    const bool in = AG.qh && quad_slot(g, cases, qoff, i, j, k, fc_groups[c][gi][t], q, slot);
+                    qslot[t] = in ? 4ll * q + slot : -1;
+                    qctr[t] = in ? ((long long)nvd + q) * A.C : 0;
+                }
+                for (int ch = 0; ch < A.C; ch++) {
+                    float gva = AG.gvattrs[(long long)v * A.C + ch];
+                    for (int t = 0; t < n; t++)
+                        if (qslot[t] >= 0) gva += AG.qh[qslot[t]] * AG.gvattrs[qctr[t] + ch];
+                    float uc[FC_MAX_GROUP_EDGES], ca[FC_MAX_GROUP_EDGES], cb[FC_MAX_GROUP_EDGES], acc = 0.f;
+                    for (int t = 0; t < n; t++) {
+                        uc[t] = attr_crossing(g, A, p0, E[t], ch, ca[t], cb[t]);
+                        acc += beta[t] * uc[t];
+                    }
+                    const float va = acc / bsum;
+                    for (int t = 0; t < n; t++) {
+                        gb[fc_groups[c][gi][t]] += gva * (uc[t] - va) / bsum;
+                        const float gu = gva * beta[t] / bsum;
+                        const float wa = E[t].sa * E[t].aa, wb = E[t].sb * E[t].ab, den = wb - wa;
+                        const float gwa = gu * (uc[t] - cb[t]) / den, gwb = gu * (ca[t] - uc[t]) / den;
+                        gs[E[t].ca] += gwa * E[t].aa;
+                        gs[E[t].cb] += gwb * E[t].ab;
+                        gan[E[t].ca] += gwa * E[t].sa;
+                        gan[E[t].cb] += gwb * E[t].sb;
+                        if (cattr) {
+                            cattr[E[t].ca * A.C + ch] += gu * (wb / den);
+                            cattr[E[t].cb * A.C + ch] -= gu * (wa / den);
+                        }
+                    }
+                }
+            }
         }
         if (cpart) {
             float4* o = cpart + 8ull * soff[f];
@@ -457,10 +579,14 @@ __global__ void __launch_bounds__(FC_THREADS) fc_cube_bwd_kernel(
 }
 
 // per grid point: the corner partials of its (up to) 8 cubes, cube offsets (dx, dy, dz) in corner order
+// (with attributes, the same for their per-corner partials, times the sigmoid's derivative at the point)
+template <bool ATTRS>
 __global__ void __launch_bounds__(FC_THREADS) fc_point_bwd_kernel(const FcGrid g, const uint8_t* __restrict__ cases,
                                                                   const uint32_t* __restrict__ soff,
                                                                   const float4* __restrict__ cpart, long long npts,
-                                                                  float* __restrict__ gx, float* __restrict__ gs) {
+                                                                  float* __restrict__ gx, float* __restrict__ gs,
+                                                                  const FcAttrs A, const float* __restrict__ cattr,
+                                                                  float* __restrict__ gattr) {
     const long long p = blockIdx.x * (long long)FC_THREADS + threadIdx.x;
     if (p >= npts) return;
     const int k = (int)(p % g.Sz), j = (int)((p / g.Sz) % (g.Ry + 1)), i = (int)(p / g.Syz);
@@ -476,6 +602,26 @@ __global__ void __launch_bounds__(FC_THREADS) fc_point_bwd_kernel(const FcGrid g
     }
     if (gx) { gx[3 * p] = ax; gx[3 * p + 1] = ay; gx[3 * p + 2] = az; }
     if (gs) gs[p] = as;
+    if constexpr (ATTRS) {
+        if (!gattr) return;
+        long long base[8];
+#pragma unroll
+        for (int c = 0; c < 8; c++) {
+            const int ci = i - (c & 1), cj = j - ((c >> 1) & 1), ck = k - (c >> 2);
+            base[c] = -1;
+            if (ci < 0 || cj < 0 || ck < 0 || ci >= g.Rx || cj >= g.Ry || ck >= g.Rz) continue;
+            const long long f = cube_id(g, ci, cj, ck);
+            if (is_surface(cases[f])) base[c] = (8ll * soff[f] + c) * A.C;
+        }
+        for (int ch = 0; ch < A.C; ch++) {
+            float acc = 0.f;
+#pragma unroll
+            for (int c = 0; c < 8; c++)
+                if (base[c] >= 0) acc += cattr[base[c] + ch];
+            const float sg = sigmoid_f(__ldg(A.a + p * A.stride + ch));
+            gattr[p * A.C + ch] = acc * (sg * (1.f - sg));
+        }
+    }
 }
 
 inline size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
@@ -513,6 +659,146 @@ FcWeights fc_weights(const float* beta, int64_t sb, const float* alpha, int64_t 
 
 inline unsigned fc_blocks(long long n) { return (unsigned)((n + FC_THREADS - 1) / FC_THREADS); }
 
+// backward workspace: quad-centre partials (training), per-corner partials of the surface cubes, then with attributes
+// the quad-centre factors (training) and the per-corner attribute partials
+struct FcWork {
+    size_t qpart, cpart, qh, cattr, total;
+};
+
+FcWork fc_work(const unsigned long long* totals_host4, int training, int C) {
+    const unsigned long long nq = training ? totals_host4[2] : 0, ns = totals_host4[3];
+    FcWork w;
+    w.qpart = 0;
+    w.cpart = align256(4 * nq * sizeof(float4));
+    if (!C) {
+        w.qh = w.cattr = w.total = w.cpart + 8 * ns * sizeof(float4);
+        return w;
+    }
+    w.qh = w.cpart + align256(8 * ns * sizeof(float4));
+    w.cattr = w.qh + align256(4 * nq * sizeof(float));
+    w.total = w.cattr + 8 * ns * C * sizeof(float);
+    return w;
+}
+
+bool fc_attrs_ok(const char* fn, const float* attrs, int64_t stride, int32_t C) {
+    if (!attrs) { gs_set_error("%s: NULL attributes", fn); return false; }
+    if (C < 1 || stride < C) {
+        gs_set_error("%s: %d attribute channels with row stride %lld: need C >= 1 and stride >= C", fn, C,
+                     (long long)stride);
+        return false;
+    }
+    return true;
+}
+
+int32_t fc_write(const float* x, const float* s, const FcWeights& W, int32_t Rx, int32_t Ry, int32_t Rz,
+                 int32_t training, const unsigned long long* totals_host4, float* verts, int64_t* faces, float* ldev,
+                 const FcAttrs& A, float* vattrs, void* scratch, cudaStream_t st) {
+    const char* fn = A.C ? "flexicubes_write_attrs" : "flexicubes_write";
+    if (!fc_dims_ok(Rx, Ry, Rz)) { gs_set_error("%s: unsupported grid %dx%dx%d", fn, Rx, Ry, Rz); return 1; }
+    if (!totals_host4) { gs_set_error("%s: NULL totals", fn); return 1; }
+    const unsigned long long nvd = totals_host4[0], nq = totals_host4[2];
+    if (nvd + nq >= (1ull << 31)) { gs_set_error("flexicubes: %llu vertices: too many", nvd + nq); return 1; }
+    if (nvd == 0) return 0;
+    if (!x || !s || !scratch || !verts || !ldev || (nq && !faces) || (A.C && !vattrs)) {
+        gs_set_error("%s: NULL pointer", fn);
+        return 1;
+    }
+    const FcGrid g = fc_grid(Rx, Ry, Rz);
+    FcScratch S = fc_scratch(scratch, g.F);
+    if (A.C)
+        fc_vertex_kernel<true><<<fc_blocks(g.F), FC_THREADS, 0, st>>>(x, s, g, W, A, S.cases, S.off[0], S.off[1],
+                                                                      verts, ldev, vattrs);
+    else
+        fc_vertex_kernel<false><<<fc_blocks(g.F), FC_THREADS, 0, st>>>(x, s, g, W, A, S.cases, S.off[0], S.off[1],
+                                                                       verts, ldev, nullptr);
+    gs_count_launches(1);
+    GS_CUDA_CHECK(cudaGetLastError());
+    if (nq) {
+        if (A.C)
+            fc_quad_kernel<true><<<fc_blocks(g.F), FC_THREADS, 0, st>>>(s, g, W, S.cases, S.off[0], S.off[2],
+                                                                        (uint32_t)nvd, training, verts, faces, A.C,
+                                                                        vattrs);
+        else
+            fc_quad_kernel<false><<<fc_blocks(g.F), FC_THREADS, 0, st>>>(s, g, W, S.cases, S.off[0], S.off[2],
+                                                                         (uint32_t)nvd, training, verts, faces, 0,
+                                                                         nullptr);
+        gs_count_launches(1);
+        GS_CUDA_CHECK(cudaGetLastError());
+    }
+    return 0;
+}
+
+int32_t fc_backward(const float* x, const float* s, const FcWeights& W, int32_t Rx, int32_t Ry, int32_t Rz,
+                    int32_t training, const unsigned long long* totals_host4, const float* verts,
+                    const float* grad_verts, const float* grad_ldev, float* grad_x, float* grad_s, float* grad_beta,
+                    float* grad_alpha, float* grad_gamma, const FcAttrs& A, const float* vattrs,
+                    const float* grad_vattrs, float* grad_attrs, void* scratch, void* workspace, cudaStream_t st) {
+    const char* fn = A.C ? "flexicubes_backward_attrs" : "flexicubes_backward";
+    if (!fc_dims_ok(Rx, Ry, Rz)) { gs_set_error("%s: unsupported grid %dx%dx%d", fn, Rx, Ry, Rz); return 1; }
+    if (!totals_host4 || !x || !s || !scratch) { gs_set_error("%s: NULL pointer", fn); return 1; }
+    if ((grad_beta && !W.beta) || (grad_alpha && !W.alpha) || (grad_gamma && !W.gamma)) {
+        gs_set_error("%s: a weight gradient needs its weight", fn);
+        return 1;
+    }
+    const unsigned long long nvd = totals_host4[0], nq = totals_host4[2];
+    const FcGrid g = fc_grid(Rx, Ry, Rz);
+    const long long npts = (long long)(Rx + 1) * (Ry + 1) * (Rz + 1);
+    if (nvd == 0) {   // empty mesh: every gradient is zero
+        if (grad_x) GS_CUDA_CHECK(cudaMemsetAsync(grad_x, 0, 12 * npts, st));
+        if (grad_s) GS_CUDA_CHECK(cudaMemsetAsync(grad_s, 0, 4 * npts, st));
+        if (grad_beta) GS_CUDA_CHECK(cudaMemsetAsync(grad_beta, 0, 48 * g.F, st));
+        if (grad_alpha) GS_CUDA_CHECK(cudaMemsetAsync(grad_alpha, 0, 32 * g.F, st));
+        if (grad_gamma) GS_CUDA_CHECK(cudaMemsetAsync(grad_gamma, 0, 4 * g.F, st));
+        if (grad_attrs) GS_CUDA_CHECK(cudaMemsetAsync(grad_attrs, 0, 4 * npts * A.C, st));
+        return 0;
+    }
+    if (!verts || !grad_verts || !grad_ldev || !workspace || (A.C && (!vattrs || !grad_vattrs))) {
+        gs_set_error("%s: NULL pointer", fn);
+        return 1;
+    }
+    FcScratch S = fc_scratch(scratch, g.F);
+    const FcWork L = fc_work(totals_host4, training, A.C);
+    char* w = (char*)workspace;
+    float4* qpart = (training && nq) ? (float4*)(w + L.qpart) : nullptr;
+    float4* cpart = (grad_x || grad_s || grad_attrs) ? (float4*)(w + L.cpart) : nullptr;
+    const FcAttrGrads AG{grad_vattrs, qpart && A.C ? (const float*)(w + L.qh) : nullptr,
+                         grad_attrs ? (float*)(w + L.cattr) : nullptr};
+    if (qpart) {
+        if (A.C)
+            fc_quad_bwd_kernel<true><<<fc_blocks(g.F), FC_THREADS, 0, st>>>(
+                s, g, W, S.cases, S.off[0], S.off[2], (uint32_t)nvd, verts, grad_verts, qpart, A.C, vattrs,
+                grad_vattrs, (float*)AG.qh);
+        else
+            fc_quad_bwd_kernel<false><<<fc_blocks(g.F), FC_THREADS, 0, st>>>(
+                s, g, W, S.cases, S.off[0], S.off[2], (uint32_t)nvd, verts, grad_verts, qpart, 0, nullptr, nullptr,
+                nullptr);
+        gs_count_launches(1);
+        GS_CUDA_CHECK(cudaGetLastError());
+    }
+    if (A.C)
+        fc_cube_bwd_kernel<true><<<fc_blocks(g.F), FC_THREADS, 0, st>>>(
+            x, s, g, W, S.cases, S.off[0], S.off[1], S.off[2], S.off[3], grad_verts, grad_ldev, qpart, cpart,
+            grad_beta, grad_alpha, grad_gamma, A, AG, (uint32_t)nvd);
+    else
+        fc_cube_bwd_kernel<false><<<fc_blocks(g.F), FC_THREADS, 0, st>>>(
+            x, s, g, W, S.cases, S.off[0], S.off[1], S.off[2], S.off[3], grad_verts, grad_ldev, qpart, cpart,
+            grad_beta, grad_alpha, grad_gamma, A, AG, (uint32_t)nvd);
+    gs_count_launches(1);
+    GS_CUDA_CHECK(cudaGetLastError());
+    if (cpart) {
+        if (A.C)
+            fc_point_bwd_kernel<true><<<fc_blocks(npts), FC_THREADS, 0, st>>>(g, S.cases, S.off[3], cpart, npts,
+                                                                              grad_x, grad_s, A, AG.cattr,
+                                                                              grad_attrs);
+        else
+            fc_point_bwd_kernel<false><<<fc_blocks(npts), FC_THREADS, 0, st>>>(g, S.cases, S.off[3], cpart, npts,
+                                                                               grad_x, grad_s, A, nullptr, nullptr);
+        gs_count_launches(1);
+        GS_CUDA_CHECK(cudaGetLastError());
+    }
+    return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -543,34 +829,32 @@ int32_t ngp_b200_flexicubes_write(const float* x, const float* s, const float* b
                                   int32_t Rx, int32_t Ry, int32_t Rz, double weight_scale, int32_t training,
                                   const unsigned long long* totals_host4, float* verts, int64_t* faces, float* ldev,
                                   void* scratch, void* stream) {
-    cudaStream_t st = (cudaStream_t)stream;
-    if (!fc_dims_ok(Rx, Ry, Rz)) { gs_set_error("flexicubes_write: unsupported grid %dx%dx%d", Rx, Ry, Rz); return 1; }
-    if (!totals_host4) { gs_set_error("flexicubes_write: NULL totals"); return 1; }
-    const unsigned long long nvd = totals_host4[0], nq = totals_host4[2];
-    if (nvd + nq >= (1ull << 31)) { gs_set_error("flexicubes: %llu vertices: too many", nvd + nq); return 1; }
-    if (nvd == 0) return 0;
-    if (!x || !s || !scratch || !verts || !ldev || (nq && !faces)) {
-        gs_set_error("flexicubes_write: NULL pointer");
-        return 1;
-    }
-    const FcGrid g = fc_grid(Rx, Ry, Rz);
-    const FcWeights W = fc_weights(beta, beta_stride, alpha, alpha_stride, gamma, gamma_stride, weight_scale);
-    FcScratch S = fc_scratch(scratch, g.F);
-    fc_vertex_kernel<<<fc_blocks(g.F), FC_THREADS, 0, st>>>(x, s, g, W, S.cases, S.off[0], S.off[1], verts, ldev);
-    gs_count_launches(1);
-    GS_CUDA_CHECK(cudaGetLastError());
-    if (nq) {
-        fc_quad_kernel<<<fc_blocks(g.F), FC_THREADS, 0, st>>>(s, g, W, S.cases, S.off[0], S.off[2], (uint32_t)nvd,
-                                                              training, verts, faces);
-        gs_count_launches(1);
-        GS_CUDA_CHECK(cudaGetLastError());
-    }
-    return 0;
+    return fc_write(x, s, fc_weights(beta, beta_stride, alpha, alpha_stride, gamma, gamma_stride, weight_scale), Rx,
+                    Ry, Rz, training, totals_host4, verts, faces, ldev, FcAttrs{nullptr, 0, 0}, nullptr, scratch,
+                    (cudaStream_t)stream);
+}
+
+int32_t ngp_b200_flexicubes_write_attrs(const float* x, const float* s, const float* beta, int64_t beta_stride,
+                                        const float* alpha, int64_t alpha_stride, const float* gamma,
+                                        int64_t gamma_stride, int32_t Rx, int32_t Ry, int32_t Rz, double weight_scale,
+                                        int32_t training, const unsigned long long* totals_host4, float* verts,
+                                        int64_t* faces, float* ldev, const float* attrs, int64_t attr_row_stride,
+                                        int32_t C, float* vattrs, void* scratch, void* stream) {
+    if (!fc_attrs_ok("flexicubes_write_attrs", attrs, attr_row_stride, C)) return 1;
+    return fc_write(x, s, fc_weights(beta, beta_stride, alpha, alpha_stride, gamma, gamma_stride, weight_scale), Rx,
+                    Ry, Rz, training, totals_host4, verts, faces, ldev, FcAttrs{attrs, attr_row_stride, C}, vattrs,
+                    scratch, (cudaStream_t)stream);
 }
 
 size_t ngp_b200_flexicubes_backward_workspace_bytes(const unsigned long long* totals_host4, int32_t training) {
     if (!totals_host4) return 0;
-    return align256((training ? 4 * totals_host4[2] : 0) * sizeof(float4)) + 8 * totals_host4[3] * sizeof(float4);
+    return fc_work(totals_host4, training, 0).total;
+}
+
+size_t ngp_b200_flexicubes_backward_attrs_workspace_bytes(const unsigned long long* totals_host4, int32_t training,
+                                                          int32_t C) {
+    if (!totals_host4 || C < 1) return 0;
+    return fc_work(totals_host4, training, C).total;
 }
 
 int32_t ngp_b200_flexicubes_backward(const float* x, const float* s, const float* beta, int64_t beta_stride,
@@ -580,47 +864,27 @@ int32_t ngp_b200_flexicubes_backward(const float* x, const float* s, const float
                                      const float* grad_verts, const float* grad_ldev, float* grad_x, float* grad_s,
                                      float* grad_beta, float* grad_alpha, float* grad_gamma, void* scratch,
                                      void* workspace, void* stream) {
-    cudaStream_t st = (cudaStream_t)stream;
-    if (!fc_dims_ok(Rx, Ry, Rz)) { gs_set_error("flexicubes_backward: unsupported grid %dx%dx%d", Rx, Ry, Rz); return 1; }
-    if (!totals_host4 || !x || !s || !scratch) { gs_set_error("flexicubes_backward: NULL pointer"); return 1; }
-    if ((grad_beta && !beta) || (grad_alpha && !alpha) || (grad_gamma && !gamma)) {
-        gs_set_error("flexicubes_backward: a weight gradient needs its weight");
-        return 1;
-    }
-    const unsigned long long nvd = totals_host4[0], nq = totals_host4[2];
-    const FcGrid g = fc_grid(Rx, Ry, Rz);
-    const long long npts = (long long)(Rx + 1) * (Ry + 1) * (Rz + 1);
-    if (nvd == 0) {   // empty mesh: every gradient is zero
-        if (grad_x) GS_CUDA_CHECK(cudaMemsetAsync(grad_x, 0, 12 * npts, st));
-        if (grad_s) GS_CUDA_CHECK(cudaMemsetAsync(grad_s, 0, 4 * npts, st));
-        if (grad_beta) GS_CUDA_CHECK(cudaMemsetAsync(grad_beta, 0, 48 * g.F, st));
-        if (grad_alpha) GS_CUDA_CHECK(cudaMemsetAsync(grad_alpha, 0, 32 * g.F, st));
-        if (grad_gamma) GS_CUDA_CHECK(cudaMemsetAsync(grad_gamma, 0, 4 * g.F, st));
-        return 0;
-    }
-    if (!verts || !grad_verts || !grad_ldev || !workspace) { gs_set_error("flexicubes_backward: NULL pointer"); return 1; }
-    const FcWeights W = fc_weights(beta, beta_stride, alpha, alpha_stride, gamma, gamma_stride, weight_scale);
-    FcScratch S = fc_scratch(scratch, g.F);
-    float4* qpart = (training && nq) ? (float4*)workspace : nullptr;
-    float4* cpart = (grad_x || grad_s)
-        ? (float4*)((char*)workspace + align256((training ? 4 * nq : 0) * sizeof(float4))) : nullptr;
-    if (qpart) {
-        fc_quad_bwd_kernel<<<fc_blocks(g.F), FC_THREADS, 0, st>>>(s, g, W, S.cases, S.off[0], S.off[2],
-                                                                  (uint32_t)nvd, verts, grad_verts, qpart);
-        gs_count_launches(1);
-        GS_CUDA_CHECK(cudaGetLastError());
-    }
-    fc_cube_bwd_kernel<<<fc_blocks(g.F), FC_THREADS, 0, st>>>(x, s, g, W, S.cases, S.off[0], S.off[1], S.off[2],
-                                                              S.off[3], grad_verts, grad_ldev, qpart, cpart, grad_beta,
-                                                              grad_alpha, grad_gamma);
-    gs_count_launches(1);
-    GS_CUDA_CHECK(cudaGetLastError());
-    if (cpart) {
-        fc_point_bwd_kernel<<<fc_blocks(npts), FC_THREADS, 0, st>>>(g, S.cases, S.off[3], cpart, npts, grad_x, grad_s);
-        gs_count_launches(1);
-        GS_CUDA_CHECK(cudaGetLastError());
-    }
-    return 0;
+    return fc_backward(x, s, fc_weights(beta, beta_stride, alpha, alpha_stride, gamma, gamma_stride, weight_scale),
+                       Rx, Ry, Rz, training, totals_host4, verts, grad_verts, grad_ldev, grad_x, grad_s, grad_beta,
+                       grad_alpha, grad_gamma, FcAttrs{nullptr, 0, 0}, nullptr, nullptr, nullptr, scratch, workspace,
+                       (cudaStream_t)stream);
+}
+
+int32_t ngp_b200_flexicubes_backward_attrs(const float* x, const float* s, const float* beta, int64_t beta_stride,
+                                           const float* alpha, int64_t alpha_stride, const float* gamma,
+                                           int64_t gamma_stride, int32_t Rx, int32_t Ry, int32_t Rz,
+                                           double weight_scale, int32_t training,
+                                           const unsigned long long* totals_host4, const float* verts,
+                                           const float* grad_verts, const float* grad_ldev, float* grad_x,
+                                           float* grad_s, float* grad_beta, float* grad_alpha, float* grad_gamma,
+                                           const float* attrs, int64_t attr_row_stride, int32_t C,
+                                           const float* vattrs, const float* grad_vattrs, float* grad_attrs,
+                                           void* scratch, void* workspace, void* stream) {
+    if (!fc_attrs_ok("flexicubes_backward_attrs", attrs, attr_row_stride, C)) return 1;
+    return fc_backward(x, s, fc_weights(beta, beta_stride, alpha, alpha_stride, gamma, gamma_stride, weight_scale),
+                       Rx, Ry, Rz, training, totals_host4, verts, grad_verts, grad_ldev, grad_x, grad_s, grad_beta,
+                       grad_alpha, grad_gamma, FcAttrs{attrs, attr_row_stride, C}, vattrs, grad_vattrs, grad_attrs,
+                       scratch, workspace, (cudaStream_t)stream);
 }
 
 }  // extern "C"

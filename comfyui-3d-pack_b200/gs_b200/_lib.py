@@ -158,12 +158,22 @@ lib.ngp_b200_flexicubes_backward_workspace_bytes.restype = C.c_size_t
 lib.ngp_b200_flexicubes_backward_workspace_bytes.argtypes = [_U4, _I]
 lib.ngp_b200_flexicubes_backward.restype = _I
 lib.ngp_b200_flexicubes_backward.argtypes = [_P, _P, _P, _L, _P, _L, _P, _L, _I, _I, _I, _D, _I, _U4] + [_P] * 11
+lib.ngp_b200_flexicubes_write_attrs.restype = _I
+lib.ngp_b200_flexicubes_write_attrs.argtypes = [_P, _P, _P, _L, _P, _L, _P, _L, _I, _I, _I, _D, _I, _U4, _P, _P, _P,
+                                                _P, _L, _I, _P, _P, _P]
+lib.ngp_b200_flexicubes_backward_attrs_workspace_bytes.restype = C.c_size_t
+lib.ngp_b200_flexicubes_backward_attrs_workspace_bytes.argtypes = [_U4, _I, _I]
+lib.ngp_b200_flexicubes_backward_attrs.restype = _I
+lib.ngp_b200_flexicubes_backward_attrs.argtypes = [_P, _P, _P, _L, _P, _L, _P, _L, _I, _I, _I, _D, _I, _U4] + \
+    [_P] * 8 + [_P, _L, _I] + [_P] * 6
 NGP_EXPORTS = ["ngp_b200_mlp2_supported", "ngp_b200_mlp2_fwd", "ngp_b200_mlp2_bwd","ngp_b200_grid_encode_fwd", "ngp_b200_grid_encode_bwd", "ngp_b200_grid_tv_grad", "ngp_b200_march_scratch_bytes",
                "ngp_b200_march_count", "ngp_b200_march_write", "ngp_b200_ray_ranges", "ngp_b200_weights_fwd",
                "ngp_b200_weights_bwd", "ngp_b200_accumulate_fwd", "ngp_b200_accumulate_bwd",
                "ngp_b200_mcubes_scratch_bytes", "ngp_b200_mcubes_count", "ngp_b200_mcubes_write",
                "ngp_b200_flexicubes_scratch_bytes", "ngp_b200_flexicubes_count", "ngp_b200_flexicubes_write",
-               "ngp_b200_flexicubes_backward_workspace_bytes", "ngp_b200_flexicubes_backward"]
+               "ngp_b200_flexicubes_backward_workspace_bytes", "ngp_b200_flexicubes_backward",
+               "ngp_b200_flexicubes_write_attrs", "ngp_b200_flexicubes_backward_attrs_workspace_bytes",
+               "ngp_b200_flexicubes_backward_attrs"]
 
 lib.gs_b200_activate.restype = _I
 lib.gs_b200_activate.argtypes = [_I, _P, _P, _P, _P, _P, _P, _P]

@@ -3,7 +3,9 @@
 `marching_cubes` replaces PyMCubes' `marching_cubes(volume, iso)` in the density-to-mesh step of the Instant-NGP node
 (mesh_processer/mesh_utils.py:509) and LGM's converter (nerf_marching_cubes_converter.py:245); its case table is
 csrc/mc_table.cuh, written by scripts/gen_mc_table.py.  `FlexiCubes` replaces the FlexiCubes class of the FlexiCubes
-node, CRM and InstantMesh; its case table is csrc/fc_table.cuh, written by scripts/gen_fc_table.py.  No CPU path."""
+node, CRM and InstantMesh; its case table is csrc/fc_table.cuh, written by scripts/gen_fc_table.py.
+`TrellisFlexiCubes` replaces the FlexiCubes of TRELLIS and Stable3DGen's mesh decoders (cube2mesh.py), the same
+extraction with per-vertex colours.  No CPU path."""
 import ctypes as C
 
 import torch
@@ -82,14 +84,28 @@ def _weight_arg(w, cols, F, name):
     return w, w.stride(0)
 
 
+def _attr_arg(a, P):
+    """(tensor with unit column stride, row stride, C) of raw vertex attributes [P,C] such as v_attrs_d[..., 4:]."""
+    if a is None:
+        return None, 0, 0
+    if a.dim() != 2 or a.shape[0] != P or a.shape[1] < 1:
+        raise AssertionError("'voxelgrid_colors' should be a tensor of shape (num_vertices, C)")
+    if a.dtype != torch.float32 or a.stride(1) != 1 or a.stride(0) < a.shape[1]:
+        a = a.float().contiguous()
+    return a, a.stride(0), a.shape[1]
+
+
 class _FlexiCubesFn(torch.autograd.Function):
+    """Both extractions: without attributes (attrs None) through ngp_b200_flexicubes_{write,backward}, with them
+    through the *_attrs entries.  Returns (verts, faces, L_dev, vertex attributes or None)."""
     @staticmethod
-    def forward(ctx, x, s, beta, alpha, gamma, R, ws, training):
+    def forward(ctx, x, s, beta, alpha, gamma, attrs, R, ws, training):
         dev = x.device
         F = R[0] * R[1] * R[2]
         (beta, sb), (alpha, sa), (gamma, sg) = (_weight_arg(beta, 12, F, "beta_fx12"),
                                                 _weight_arg(alpha, 8, F, "alpha_fx8"),
                                                 _weight_arg(gamma, 0, F, "gamma_f"))
+        attrs, sc, nc = _attr_arg(attrs, x.shape[0])
         opt = lambda t: _P(t) if t is not None else None
         with torch.cuda.device(dev):
             stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
@@ -102,19 +118,25 @@ class _FlexiCubesFn(torch.autograd.Function):
             verts = torch.empty((nv, 3), dtype=torch.float32, device=dev)
             faces = torch.empty(((4 if training else 2) * nq if nvd else 0, 3), dtype=torch.int64, device=dev)
             ldev = torch.empty((nl if nvd else 0,), dtype=torch.float32, device=dev)
-            _lib.check(_lib.lib.ngp_b200_flexicubes_write(
-                _P(x), _P(s), opt(beta), sb, opt(alpha), sa, opt(gamma), sg, *R, float(ws), int(training), host,
-                _P(verts), _P(faces), _P(ldev), _P(scratch), stream))
+            args = (_P(x), _P(s), opt(beta), sb, opt(alpha), sa, opt(gamma), sg, *R, float(ws), int(training), host,
+                    _P(verts), _P(faces), _P(ldev))
+            if attrs is None:
+                vattrs = None
+                _lib.check(_lib.lib.ngp_b200_flexicubes_write(*args, _P(scratch), stream))
+            else:
+                vattrs = torch.empty((nv, nc), dtype=torch.float32, device=dev)
+                _lib.check(_lib.lib.ngp_b200_flexicubes_write_attrs(*args, _P(attrs), sc, nc, _P(vattrs),
+                                                                     _P(scratch), stream))
         ctx.mark_non_differentiable(faces)
-        ctx.save_for_backward(x, s, beta, alpha, gamma, verts, scratch)
-        ctx.meta = (R, ws, training, (nvd, nl, nq, ns), (sb, sa, sg))
-        return verts, faces, ldev
+        ctx.save_for_backward(x, s, beta, alpha, gamma, attrs, verts, vattrs, scratch)
+        ctx.meta = (R, ws, training, (nvd, nl, nq, ns), (sb, sa, sg, sc, nc))
+        return verts, faces, ldev, vattrs
 
     @staticmethod
     @torch.autograd.function.once_differentiable
-    def backward(ctx, gverts, _gfaces, gldev):
-        x, s, beta, alpha, gamma, verts, scratch = ctx.saved_tensors
-        R, ws, training, totals, (sb, sa, sg) = ctx.meta
+    def backward(ctx, gverts, _gfaces, gldev, gvattrs):
+        x, s, beta, alpha, gamma, attrs, verts, vattrs, scratch = ctx.saved_tensors
+        R, ws, training, totals, (sb, sa, sg, sc, nc) = ctx.meta
         need = ctx.needs_input_grad
         dev = x.device
         F = R[0] * R[1] * R[2]
@@ -125,16 +147,23 @@ class _FlexiCubesFn(torch.autograd.Function):
         new = lambda want, shape: torch.empty(shape, dtype=torch.float32, device=dev) if want else None
         gx, gs = new(need[0], x.shape), new(need[1], s.shape)
         gb, ga, gg = new(need[2], (F, 12)), new(need[3], (F, 8)), new(need[4], (F,))
+        gat = new(attrs is not None and need[5], (x.shape[0], nc))
         opt = lambda t: _P(t) if t is not None else None
         with torch.cuda.device(dev):
             stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-            ws_bytes = int(_lib.lib.ngp_b200_flexicubes_backward_workspace_bytes(host, int(training)))
-            work = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
-            _lib.check(_lib.lib.ngp_b200_flexicubes_backward(
-                _P(x), _P(s), opt(beta), sb, opt(alpha), sa, opt(gamma), sg, *R, float(ws), int(training), host,
-                _P(verts), _P(gverts), _P(gldev), opt(gx), opt(gs), opt(gb), opt(ga), opt(gg), _P(scratch), _P(work),
-                stream))
-        return gx, gs, gb, ga, gg, None, None, None
+            args = (_P(x), _P(s), opt(beta), sb, opt(alpha), sa, opt(gamma), sg, *R, float(ws), int(training), host,
+                    _P(verts), _P(gverts), _P(gldev), opt(gx), opt(gs), opt(gb), opt(ga), opt(gg))
+            if attrs is None:
+                ws_bytes = int(_lib.lib.ngp_b200_flexicubes_backward_workspace_bytes(host, int(training)))
+                work = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
+                _lib.check(_lib.lib.ngp_b200_flexicubes_backward(*args, _P(scratch), _P(work), stream))
+            else:
+                gvattrs = torch.zeros_like(vattrs) if gvattrs is None else gvattrs.float().contiguous()
+                ws_bytes = int(_lib.lib.ngp_b200_flexicubes_backward_attrs_workspace_bytes(host, int(training), nc))
+                work = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
+                _lib.check(_lib.lib.ngp_b200_flexicubes_backward_attrs(
+                    *args, _P(attrs), sc, nc, _P(vattrs), _P(gvattrs), opt(gat), _P(scratch), _P(work), stream))
+        return gx, gs, gb, ga, gg, gat, None, None, None
 
 
 class FlexiCubes:
@@ -188,4 +217,55 @@ class FlexiCubes:
         self._check_cubes(cube_fx8, R)
         x = x_nx3.float().contiguous()
         s = s_n.reshape(-1).float().contiguous()
-        return _FlexiCubesFn.apply(x, s, beta_fx12, alpha_fx8, gamma_f, R, float(self.weight_scale), bool(training))
+        return _FlexiCubesFn.apply(x, s, beta_fx12, alpha_fx8, gamma_f, None, R, float(self.weight_scale),
+                                   bool(training))[:3]
+
+
+class TrellisFlexiCubes:
+    """FlexiCubes mesh extraction with vertex attributes on the GPU: a drop-in for the FlexiCubes of TRELLIS and
+    Stable3DGen (trellis/representations/mesh/flexicubes), which SparseFeatures2Mesh calls once per shape.  The
+    geometry is FlexiCubes' (same kernels, same bits); voxelgrid_colors [P,C] go through a sigmoid and are
+    interpolated to each dual vertex with the same weights as its position, and in training to each quad centre with
+    the same gamma-weighted means.  qef_reg_scale is accepted and unused, as in the reference.  No CPU path."""
+
+    def __init__(self, device="cuda"):
+        self.device = torch.device(device)
+        self._fc = FlexiCubes(device=device)
+
+    def __call__(self, voxelgrid_vertices, scalar_field, cube_idx, resolution, qef_reg_scale=1e-3,
+                 weight_scale=0.99, beta=None, alpha=None, gamma_f=None, voxelgrid_colors=None, training=False):
+        """(vertices fp32 [V,3], faces int64 [T,3], L_dev fp32 [E], vertices_color fp32 [V,C] or None), on the current
+        stream with one host read; differentiable in the vertices, the scalar field, the three raw weights and the
+        raw colours."""
+        def shaped(t, shape):
+            return torch.is_tensor(t) and t.dim() == len(shape) and all(
+                d is None or t.shape[i] == d for i, d in enumerate(shape))
+
+        if not shaped(voxelgrid_vertices, (None, 3)):
+            raise AssertionError("'voxelgrid_vertices' should be a tensor of shape (num_vertices, 3)")
+        P = voxelgrid_vertices.shape[0]
+        if not shaped(scalar_field, (P,)):
+            raise AssertionError("'scalar_field' should be a tensor of shape (num_vertices,)")
+        if not shaped(cube_idx, (None, 8)):
+            raise AssertionError("'cube_idx' should be a tensor of shape (num_cubes, 8)")
+        F = cube_idx.shape[0]
+        for name, t, shape, text in (("beta", beta, (F, 12), "(num_cubes, 12)"),
+                                     ("alpha", alpha, (F, 8), "(num_cubes, 8)"),
+                                     ("gamma_f", gamma_f, (F,), "(num_cubes,)")):
+            if t is not None and not shaped(t, shape):
+                raise AssertionError(f"'{name}' should be a tensor of shape {text}")
+        if voxelgrid_colors is not None and not shaped(voxelgrid_colors, (P, None)):
+            raise AssertionError("'voxelgrid_colors' should be a tensor of shape (num_vertices, C)")
+        for name, t in (("voxelgrid_vertices", voxelgrid_vertices), ("scalar_field", scalar_field),
+                        ("cube_idx", cube_idx), ("beta", beta), ("alpha", alpha), ("gamma_f", gamma_f),
+                        ("voxelgrid_colors", voxelgrid_colors)):
+            if t is not None and not t.is_cuda:
+                raise TypeError(f"TrellisFlexiCubes: {name} must be a CUDA tensor (gs_b200 has no CPU path)")
+        R = _res3(resolution)
+        if P != (R[0] + 1) * (R[1] + 1) * (R[2] + 1):
+            raise ValueError(f"TrellisFlexiCubes: {P} grid points do not make the grid of resolution {R}")
+        self._fc._check_cubes(cube_idx, R)
+        x = voxelgrid_vertices.float().contiguous()
+        s = scalar_field.float().contiguous()
+        return _FlexiCubesFn.apply(x, s, beta, alpha, gamma_f, voxelgrid_colors, R, float(weight_scale),
+                                   bool(training))

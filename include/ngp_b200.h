@@ -107,6 +107,32 @@ int32_t ngp_b200_flexicubes_backward(const float* x, const float* s, const float
                                      const float* grad_verts, const float* grad_ldev, float* grad_x, float* grad_s,
                                      float* grad_beta, float* grad_alpha, float* grad_gamma, void* scratch,
                                      void* workspace, void* stream);
+/* The same extraction with C >= 1 vertex attributes (the TRELLIS / Stable3DGen FlexiCubes' voxelgrid_colors): raw
+ * attrs[P,C] are fp32 rows with row stride attr_row_stride >= C (unit column stride).  Each dual vertex gets
+ * sum(beta * uc) / sum(beta) per channel, uc the crossing of sigmoid(attrs) at the edge's ends with the same end
+ * weights as its position; training centres get the same gamma-weighted diagonal means.  write_attrs writes
+ * vattrs[V,C] next to what write writes, which it writes with the same bits.  backward_attrs takes vattrs and
+ * grad_vattrs[V,C] and, besides write's gradients (which now include the attributes' terms), writes grad_attrs[P,C]
+ * (contiguous, zero off the surface; NULL = not wanted); workspace >= flexicubes_backward_attrs_workspace_bytes.
+ * count is shared: topology does not depend on the attributes. */
+int32_t ngp_b200_flexicubes_write_attrs(const float* x, const float* s, const float* beta, int64_t beta_stride,
+                                        const float* alpha, int64_t alpha_stride, const float* gamma,
+                                        int64_t gamma_stride, int32_t Rx, int32_t Ry, int32_t Rz, double weight_scale,
+                                        int32_t training, const unsigned long long* totals_host4, float* verts,
+                                        int64_t* faces, float* ldev, const float* attrs, int64_t attr_row_stride,
+                                        int32_t C, float* vattrs, void* scratch, void* stream);
+size_t ngp_b200_flexicubes_backward_attrs_workspace_bytes(const unsigned long long* totals_host4, int32_t training,
+                                                          int32_t C);
+int32_t ngp_b200_flexicubes_backward_attrs(const float* x, const float* s, const float* beta, int64_t beta_stride,
+                                           const float* alpha, int64_t alpha_stride, const float* gamma,
+                                           int64_t gamma_stride, int32_t Rx, int32_t Ry, int32_t Rz,
+                                           double weight_scale, int32_t training,
+                                           const unsigned long long* totals_host4, const float* verts,
+                                           const float* grad_verts, const float* grad_ldev, float* grad_x,
+                                           float* grad_s, float* grad_beta, float* grad_alpha, float* grad_gamma,
+                                           const float* attrs, int64_t attr_row_stride, int32_t C,
+                                           const float* vattrs, const float* grad_vattrs, float* grad_attrs,
+                                           void* scratch, void* workspace, void* stream);
 #ifdef __cplusplus
 }
 #endif
