@@ -968,7 +968,7 @@ int32_t gs_b200_activate(int32_t N, const float* raw_opacities, const float* raw
     if (N > 0 && (!raw_opacities || !raw_scales || !raw_rotations || !opacities || !scales || !rotations)) { gs_set_error("activate: NULL"); return 1; }
     return gs_launch_activate(N, raw_opacities, raw_scales, raw_rotations, opacities, scales, rotations, (cudaStream_t)stream_);
 }
-int32_t gs_b200_adam_step(int32_t N, int32_t M, const float* lrs6_host, float beta1, float beta2, float eps, int32_t step,
+int32_t gs_b200_adam_step(int32_t N, int32_t M, const float* lrs6_host, double beta1, double beta2, float eps, int32_t step,
                           float grad_scale, const float* grads_packed, float* params_packed, float* exp_avg,
                           float* exp_avg_sq, void* stream_) {
     if (!lrs6_host || step < 1 || (N > 0 && (!grads_packed || !params_packed || !exp_avg || !exp_avg_sq))) { gs_set_error("adam_step: bad argument"); return 1; }

@@ -180,7 +180,7 @@ int gs_launch_image_loss(int H, int W, const float* img, const float* ref, const
                          float lambda_alpha, float scale, float* dL, float* loss_out, void* scratch, cudaStream_t s);
 
 int gs_launch_activate(int, const float*, const float*, const float*, float*, float*, float*, cudaStream_t);
-int gs_launch_adam(int, int, const float*, float, float, float, int, float, const float*, float*, float*, float*, cudaStream_t);
+int gs_launch_adam(int, int, const float*, double, double, float, int, float, const float*, float*, float*, float*, cudaStream_t);
 int gs_launch_densify_stats(int, const float*, const int32_t*, float*, float*, float*, cudaStream_t);
 
 // Segmented sort (gs_sort.cu): n segments [off[i], off[i+1]) of one key array, sorted independently in one

@@ -21,8 +21,9 @@ __constant__ float c_msw[LEVELS] = {0.0448f, 0.2856f, 0.3001f, 0.2363f, 0.1333f}
 constexpr float SSIM_C1 = 0.01f * 0.01f, SSIM_C2 = 0.03f * 0.03f;
 
 struct LossAcc {            // device accumulators of one view
-    float l1_sum, mse_sum;
-    float sums[LEVELS][3][2];     // [level][channel]{ssim_map sum, cs_map sum}
+    // the block partials meet in fp64 reds: at 1080p ~8000 fp32 atomics per sum drifted ~1e-6 relative
+    double l1_sum, mse_sum;
+    double sums[LEVELS][3][2];    // [level][channel]{ssim_map sum, cs_map sum}
     float coef[LEVELS][3][2];     // per-location coefficients {d loss / d ssim_map, d loss / d cs_map}
 };
 
@@ -57,9 +58,9 @@ prep_kernel(int npix, const float* __restrict__ img, const float* __restrict__ r
         mse = d * d;
     }
     l1 = block_sum(l1, s_red);
-    if (threadIdx.x == 0) atomicAdd(&acc->l1_sum, l1);
+    if (threadIdx.x == 0) atomicAdd(&acc->l1_sum, (double)l1);
     mse = block_sum(mse, s_red);
-    if (threadIdx.x == 0) atomicAdd(&acc->mse_sum, mse);
+    if (threadIdx.x == 0) atomicAdd(&acc->mse_sum, (double)mse);
 }
 
 // Gaussian-window statistics of one 32x8 tile of window positions, fused row + column filter through shared memory:
@@ -125,9 +126,9 @@ stats_sums_kernel(Win win, int Hs, int Ws, const float* __restrict__ X, const fl
     }
     const int c = blockIdx.z;
     ssim = block_sum(ssim, s_red);
-    if (threadIdx.x == 0) atomicAdd(&acc->sums[level][c][0], ssim);
+    if (threadIdx.x == 0) atomicAdd(&acc->sums[level][c][0], (double)ssim);
     cs = block_sum(cs, s_red);
-    if (threadIdx.x == 0) atomicAdd(&acc->sums[level][c][1], cs);
+    if (threadIdx.x == 0) atomicAdd(&acc->sums[level][c][1], (double)cs);
 }
 
 // derivatives of (b*ssim + a*cs) wrt (mu_y, E[y^2], E[xy]) -> D[3][c][yo][xo]
@@ -186,7 +187,7 @@ __global__ void coef_kernel(int H, int W, float lambda_ssim, float lambda_alpha,
     const int hs[LEVELS] = {dims0.x, dims0.y, dims0.z, dims0.w, dims4h};
     const int ws[LEVELS] = {dims1.x, dims1.y, dims1.z, dims1.w, dims4w};
     const float npix = (float)H * (float)W;
-    float loss = (1.f - lambda_ssim) * acc->l1_sum / (3.f * npix) + lambda_alpha * acc->mse_sum / npix;
+    float loss = (float)((1.0 - lambda_ssim) * acc->l1_sum / (3.0 * npix) + lambda_alpha * acc->mse_sum / npix);
     for (int l = 0; l < LEVELS; l++) for (int c = 0; c < 3; c++) { acc->coef[l][c][0] = 0.f; acc->coef[l][c][1] = 0.f; }
     if (lambda_ssim > 0.f) {
         float ms = 0.f;
@@ -194,7 +195,7 @@ __global__ void coef_kernel(int H, int W, float lambda_ssim, float lambda_alpha,
             float v[LEVELS], P = 1.f;
             for (int l = 0; l < LEVELS; l++) {
                 const float cnt = (float)(hs[l] - (WIN - 1)) * (float)(ws[l] - (WIN - 1));
-                const float mean = acc->sums[l][c][l == LEVELS - 1 ? 0 : 1] / cnt;
+                const float mean = (float)(acc->sums[l][c][l == LEVELS - 1 ? 0 : 1] / cnt);
                 v[l] = fmaxf(mean, 0.f);
                 P *= powf(v[l], c_msw[l]);
             }

@@ -27,16 +27,18 @@ activate_kernel(int N, const float* __restrict__ raw_opac, const float* __restri
 }
 
 struct AdamArgs {
-    float lr_xyz, lr_dc, lr_rest, lr_opac, lr_scale, lr_rot;
-    float beta1, beta2, eps, bias1, bias2_sqrt;     // bias1 = 1 - b1^t, bias2_sqrt = sqrt(1 - b2^t)
+    // per-group step sizes lr / (1 - b1^t); 1 - b and the bias corrections are taken in double on the host and
+    // rounded once, as torch.optim.Adam does with its Python-float hyperparameters
+    float st_xyz, st_dc, st_rest, st_opac, st_scale, st_rot;
+    float beta1, beta2, one_m_beta1, one_m_beta2, eps, bias2_sqrt;     // bias2_sqrt = sqrt(1 - b2^t)
     float grad_scale;                               // multiplies the incoming (summed) gradient, e.g. 1/world
 };
 
-__device__ __forceinline__ void adam_one(float& p, float& m, float& v, float g, float lr, const AdamArgs& a) {
-    m = a.beta1 * m + (1.f - a.beta1) * g;
-    v = a.beta2 * v + (1.f - a.beta2) * g * g;
+__device__ __forceinline__ void adam_one(float& p, float& m, float& v, float g, float step_size, const AdamArgs& a) {
+    m = a.beta1 * m + a.one_m_beta1 * g;
+    v = a.beta2 * v + a.one_m_beta2 * g * g;
     const float denom = sqrtf(v) / a.bias2_sqrt + a.eps;
-    p -= (lr / a.bias1) * (m / denom);
+    p -= step_size * (m / denom);
 }
 
 // one thread per Gaussian; grads are wrt the ACTIVATED opac/scales/rots (what the rasterizer returns)
@@ -53,30 +55,32 @@ adam_fused_kernel(int N, int M, AdamArgs a, const float* __restrict__ g_means,
 #pragma unroll
     for (int k = 0; k < 3; k++) {
         const size_t j = 3 * (size_t)i + k;
-        adam_one(p_means[j], m1[j], m2[j], a.grad_scale * g_means[j], a.lr_xyz, a);
+        adam_one(p_means[j], m1[j], m2[j], a.grad_scale * g_means[j], a.st_xyz, a);
     }
     {
         const float o = 1.0f / (1.0f + expf(-p_opac[i]));
         const float g = a.grad_scale * g_opac[i] * o * (1.f - o);
-        adam_one(p_opac[i], m1[o_op + i], m2[o_op + i], g, a.lr_opac, a);
+        adam_one(p_opac[i], m1[o_op + i], m2[o_op + i], g, a.st_opac, a);
     }
 #pragma unroll
     for (int k = 0; k < 3; k++) {
         const size_t j = 3 * (size_t)i + k;
         const float g = a.grad_scale * g_scales[j] * expf(p_scales[j]);
-        adam_one(p_scales[j], m1[o_sc + j], m2[o_sc + j], g, a.lr_scale, a);
+        adam_one(p_scales[j], m1[o_sc + j], m2[o_sc + j], g, a.st_scale, a);
     }
     {
         float r[4], g[4];
 #pragma unroll
         for (int k = 0; k < 4; k++) { r[k] = p_rots[4 * (size_t)i + k]; g[k] = a.grad_scale * g_rots[4 * (size_t)i + k]; }
-        const float nrm = fmaxf(sqrtf(r[0] * r[0] + r[1] * r[1] + r[2] * r[2] + r[3] * r[3]), 1e-12f);
-        const float inv = 1.0f / nrm;
-        const float dot = (r[0] * g[0] + r[1] * g[1] + r[2] * g[2] + r[3] * g[3]) * inv * inv;
+        // F.normalize divides by clamp_min(|r|, 1e-12): below the clamp no gradient flows through the norm, so the
+        // projection term goes and the gradient is g / 1e-12
+        const float nrm = sqrtf(r[0] * r[0] + r[1] * r[1] + r[2] * r[2] + r[3] * r[3]);
+        const float inv = 1.0f / fmaxf(nrm, 1e-12f);
+        const float dot = nrm < 1e-12f ? 0.f : (r[0] * g[0] + r[1] * g[1] + r[2] * g[2] + r[3] * g[3]) * inv * inv;
 #pragma unroll
         for (int k = 0; k < 4; k++) {
             const size_t j = 4 * (size_t)i + k;
-            adam_one(p_rots[j], m1[o_ro + j], m2[o_ro + j], (g[k] - r[k] * dot) * inv, a.lr_rot, a);
+            adam_one(p_rots[j], m1[o_ro + j], m2[o_ro + j], (g[k] - r[k] * dot) * inv, a.st_rot, a);
         }
     }
 }
@@ -94,11 +98,11 @@ adam_sh_kernel(size_t n4, int row, AdamArgs a, const float4* __restrict__ g, flo
     const float4 gv = g[i];
     // a float4 may straddle a row boundary when row = 3M is not a multiple of 4 (sh_degree 0 and 2): the wrapped
     // elements are the NEXT Gaussian's dc coefficients
-    auto lr_of = [&](int k) { int c = c0 + k; if (c >= row) c -= row; return c < 3 ? a.lr_dc : a.lr_rest; };
-    adam_one(pv.x, mv.x, vv.x, a.grad_scale * gv.x, lr_of(0), a);
-    adam_one(pv.y, mv.y, vv.y, a.grad_scale * gv.y, lr_of(1), a);
-    adam_one(pv.z, mv.z, vv.z, a.grad_scale * gv.z, lr_of(2), a);
-    adam_one(pv.w, mv.w, vv.w, a.grad_scale * gv.w, lr_of(3), a);
+    auto st_of = [&](int k) { int c = c0 + k; if (c >= row) c -= row; return c < 3 ? a.st_dc : a.st_rest; };
+    adam_one(pv.x, mv.x, vv.x, a.grad_scale * gv.x, st_of(0), a);
+    adam_one(pv.y, mv.y, vv.y, a.grad_scale * gv.y, st_of(1), a);
+    adam_one(pv.z, mv.z, vv.z, a.grad_scale * gv.z, st_of(2), a);
+    adam_one(pv.w, mv.w, vv.w, a.grad_scale * gv.w, st_of(3), a);
     p[i] = pv; m1[i] = mv; m2[i] = vv;
 }
 
@@ -108,7 +112,7 @@ adam_sh_scalar_kernel(size_t first, size_t n, int row, AdamArgs a, const float* 
                       float* __restrict__ m1, float* __restrict__ m2) {
     const size_t j = first + (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= n) return;
-    adam_one(p[j], m1[j], m2[j], a.grad_scale * g[j], (int)(j % (size_t)row) < 3 ? a.lr_dc : a.lr_rest, a);
+    adam_one(p[j], m1[j], m2[j], a.grad_scale * g[j], (int)(j % (size_t)row) < 3 ? a.st_dc : a.st_rest, a);
 }
 
 __global__ void __launch_bounds__(256)
@@ -119,7 +123,8 @@ densify_stats_kernel(int N, const float* __restrict__ g_means2D, const int32_t* 
     const int r = radii[i];
     if (r <= 0) return;
     const float gx = g_means2D[3 * (size_t)i], gy = g_means2D[3 * (size_t)i + 1];
-    grad_accum[i] += sqrtf(gx * gx + gy * gy);
+    // the norm in double: the squares neither overflow (|g| > 1.8e19) nor flush to zero (|g| < 1e-23)
+    grad_accum[i] += (float)sqrt((double)gx * gx + (double)gy * gy);
     denom[i] += 1.0f;
     max_radii[i] = fmaxf(max_radii[i], (float)r);
 }
@@ -135,13 +140,15 @@ int gs_launch_activate(int N, const float* raw_opac, const float* raw_scales, co
     return 0;
 }
 
-int gs_launch_adam(int N, int M, const float* lrs6, float beta1, float beta2, float eps, int step, float grad_scale,
+int gs_launch_adam(int N, int M, const float* lrs6, double beta1, double beta2, float eps, int step, float grad_scale,
                    const float* grads_packed, float* params_packed, float* m1, float* m2, cudaStream_t s) {
     if (N <= 0) return 0;
     AdamArgs a;
-    a.lr_xyz = lrs6[0]; a.lr_dc = lrs6[1]; a.lr_rest = lrs6[2]; a.lr_opac = lrs6[3]; a.lr_scale = lrs6[4]; a.lr_rot = lrs6[5];
-    a.beta1 = beta1; a.beta2 = beta2; a.eps = eps;
-    a.bias1 = 1.0f - powf(beta1, (float)step); a.bias2_sqrt = sqrtf(1.0f - powf(beta2, (float)step));
+    const double bias1 = 1.0 - pow(beta1, (double)step);
+    a.st_xyz = (float)(lrs6[0] / bias1); a.st_dc = (float)(lrs6[1] / bias1); a.st_rest = (float)(lrs6[2] / bias1);
+    a.st_opac = (float)(lrs6[3] / bias1); a.st_scale = (float)(lrs6[4] / bias1); a.st_rot = (float)(lrs6[5] / bias1);
+    a.beta1 = (float)beta1; a.beta2 = (float)beta2; a.one_m_beta1 = (float)(1.0 - beta1); a.one_m_beta2 = (float)(1.0 - beta2);
+    a.eps = eps; a.bias2_sqrt = (float)sqrt(1.0 - pow(beta2, (double)step));
     a.grad_scale = grad_scale;
     const size_t n = (size_t)N;
     const float* g = grads_packed; float* p = params_packed;

@@ -178,7 +178,7 @@ NGP_EXPORTS = ["ngp_b200_mlp2_supported", "ngp_b200_mlp2_fwd", "ngp_b200_mlp2_bw
 lib.gs_b200_activate.restype = _I
 lib.gs_b200_activate.argtypes = [_I, _P, _P, _P, _P, _P, _P, _P]
 lib.gs_b200_adam_step.restype = _I
-lib.gs_b200_adam_step.argtypes = [_I, _I, _P, _F, _F, _F, _I, _F, _P, _P, _P, _P, _P]
+lib.gs_b200_adam_step.argtypes = [_I, _I, _P, _D, _D, _F, _I, _F, _P, _P, _P, _P, _P]
 lib.gs_b200_densify_stats.restype = _I
 lib.gs_b200_densify_stats.argtypes = [_I, _P, _P, _P, _P, _P, _P]
 lib.gs_b200_densify_scratch_bytes.restype = C.c_size_t

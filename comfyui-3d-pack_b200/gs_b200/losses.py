@@ -8,8 +8,8 @@ import torch.nn.functional as F
 _MS_WEIGHTS = (0.0448, 0.2856, 0.3001, 0.2363, 0.1333)
 
 
-def _gauss_1d(size=11, sigma=1.5, device=None):
-    c = torch.arange(size, dtype=torch.float32, device=device) - size // 2
+def _gauss_1d(size=11, sigma=1.5, device=None, dtype=torch.float32):
+    c = torch.arange(size, dtype=dtype, device=device) - size // 2
     g = torch.exp(-(c ** 2) / (2 * sigma ** 2))
     return g / g.sum()
 
@@ -37,7 +37,7 @@ def ms_ssim(X, Y, data_range=1.0, size_average=True):
     """X, Y: [B,C,H,W]; the smaller side must exceed (11-1)*2^4 = 160 (as the package asserts)."""
     if min(X.shape[-2:]) <= (11 - 1) * 2 ** 4:
         raise ValueError("Image size should be larger than 160 due to the 4 downsamplings in ms-ssim")
-    win = _gauss_1d(device=X.device)
+    win = _gauss_1d(device=X.device, dtype=X.dtype)
     w = torch.tensor(_MS_WEIGHTS, device=X.device, dtype=X.dtype)
     mcs = []
     for i in range(5):

@@ -251,12 +251,13 @@ int32_t gs_b200_render_views(
  * gs_b200_activate: exp / sigmoid / normalize of :293-321 (means and SHs are used as they are).
  * gs_b200_adam_step: chain rule through those activations + torch.optim.Adam (betas, eps=1e-15 as :446) with the
  *   six per-group learning rates {xyz, f_dc, f_rest, opacity, scaling, rotation} (host array), `step` = 1-based
- *   Adam step, grad_scale multiplies the incoming gradient (1/world for averaged data-parallel gradients).
+ *   Adam step (< 1 is refused), grad_scale multiplies the incoming gradient (1/world for averaged data-parallel
+ *   gradients).  The betas are doubles: 1 - beta and the bias corrections are formed in double and rounded once.
  *   grads_packed holds gradients wrt the ACTIVATED values (what gs_b200_step_device produces).
  * gs_b200_densify_stats: add_densification_stats (:767-769) + max_radii2D update (main_3DGS.py:212) for radii > 0. */
 int32_t gs_b200_activate(int32_t N, const float* raw_opacities, const float* raw_scales, const float* raw_rotations,
                          float* opacities, float* scales, float* rotations, void* stream);
-int32_t gs_b200_adam_step(int32_t N, int32_t M, const float* lrs6_host, float beta1, float beta2, float eps, int32_t step,
+int32_t gs_b200_adam_step(int32_t N, int32_t M, const float* lrs6_host, double beta1, double beta2, float eps, int32_t step,
                           float grad_scale, const float* grads_packed, float* params_packed, float* exp_avg,
                           float* exp_avg_sq, void* stream);
 int32_t gs_b200_densify_stats(int32_t N, const float* dL_dmeans2D, const int32_t* radii, float* xyz_gradient_accum,
