@@ -190,6 +190,20 @@ lib.gs_b200_densify_apply.argtypes = [_I, _I, _P, _P, _P, _P, _I, _I, _I, _I, _P
 TRAIN_EXPORTS = ["gs_b200_activate", "gs_b200_adam_step", "gs_b200_densify_stats", "gs_b200_densify_scratch_bytes",
                  "gs_b200_densify_plan", "gs_b200_densify_apply"]
 
+SCATTER_SUM, SCATTER_MEAN, SCATTER_MAX = 0, 1, 2
+SCATTER_F32, SCATTER_I32, SCATTER_I64 = 0, 1, 2
+SCATTER_MAX_DIMS = 8
+lib.gs_b200_scatter_index_range.restype = _I
+lib.gs_b200_scatter_index_range.argtypes = [_I, _P, _I, _P, _P, _P, _P]
+lib.gs_b200_scatter_scratch_bytes.restype = C.c_size_t
+lib.gs_b200_scatter_scratch_bytes.argtypes = [_I, _I, _I, _P, _I, _P, _L]
+lib.gs_b200_scatter_forward.restype = _I
+lib.gs_b200_scatter_forward.argtypes = [_I, _I, _I, _P, _I, _L, _P, _P, _P, _P, _P, _P, _I, _P, _P, _P]
+lib.gs_b200_scatter_backward.restype = _I
+lib.gs_b200_scatter_backward.argtypes = [_I, _I, _P, _I, _L, _P, _P, _P, _P, _P, _P, _P, _P, _P]
+SCATTER_EXPORTS = ["gs_b200_scatter_index_range", "gs_b200_scatter_scratch_bytes", "gs_b200_scatter_forward",
+                   "gs_b200_scatter_backward"]
+
 NSTAGES = 9
 STAGE_NAMES = ["preprocess", "depth_sort", "scan", "emit", "tile_sort", "ranges", "composite_fwd",
                "composite_bwd", "preprocess_bwd"]
@@ -207,7 +221,7 @@ lib.gs_b200_composite_bwd_occupancy.argtypes = [C.POINTER(C.c_int32), C.POINTER(
 EXPORTS = ["gs_b200_set_grad_sink", "gs_b200_composite_bwd_occupancy", "gs_b200_image_loss", "gs_b200_step_device_train", "gs_b200_step_device_hook", "gs_b200_render_views", "gs_b200_set_tile_culling", "gs_b200_get_tile_culling", "gs_b200_step_device", "gs_b200_step_host_dev_grads", "gs_b200_launch_count", "gs_b200_profile_enable", "gs_b200_profile_read",
            "gs_b200_abi_version", "gs_b200_last_error", "gs_b200_rasterize_forward", "gs_b200_rasterize_backward",
            "gs_b200_state_free", "gs_b200_debug_sorted_keys", "gs_b200_sort_scratch_bytes",
-           "gs_b200_sort_pairs_u32", "gs_b200_knn_mean_dist2", "gs_b200_step_host"]
+           "gs_b200_sort_pairs_u32", "gs_b200_knn_mean_dist2", "gs_b200_step_host"] + SCATTER_EXPORTS
 
 
 def last_error() -> str:

@@ -150,6 +150,42 @@ int32_t gs_b200_sort_pairs_u32(uint32_t* keys, uint32_t* keys_alt, uint32_t* val
  * mean squared distance to the 3 nearest neighbours. points[N,3] -> out[N]. */
 int32_t gs_b200_knn_mean_dist2(const float* points, int32_t N, float* out, void* stream);
 
+/* ---- torch_scatter replacement (scatter_sum / scatter_add, scatter_mean, scatter_max) ---------------------------
+ * src, index and out are strided views over one shape of `ndim` dimensions (shape_host: src's shape; out has the
+ * same shape with dim_size at `dim`).  Each tensor comes with its element strides (host arrays of ndim int64); the
+ * index is int64 and has already been broadcast to src's shape, with stride 0 where it repeats.  out[.., index[e], ..]
+ * collects src[e]:
+ *   SUM (fp32)  out = (out or +0) + src in ascending position along `dim`, one fp32 add each (a fixed left fold)
+ *   SUM (int)   exact integer sums (int32 / int64 wrap)
+ *   MEAN (fp32) the fp32 sum, then one division by the number of index entries that hit the slot (at least 1)
+ *   MAX         an element replaces the running value only when strictly greater (NaN never does; among equal values
+ *               the smallest position wins); the initial value is out's (has_out) or the dtype's lowest, which becomes
+ *               0 where nothing won.  argmax: contiguous int64 [out shape], the winner's position along `dim`, or
+ *               src's size there where nothing won.
+ * has_out = 0: out's prior content is ignored.  Every index value must lie in [0, dim_size): the caller checks it
+ * first with gs_b200_scatter_index_range, which writes [min, max] of the index to range_out (2 device int64);
+ * values outside are skipped by the kernels, never written.  Sizes: fewer than 2^31 src and out elements, fewer than
+ * 2^30 index elements after dropping repeats.  No fp32 atomics: the results have the same bits on every run.
+ * scratch: gs_b200_scatter_scratch_bytes(...) bytes (0 = invalid arguments, see gs_b200_last_error).
+ * Backward (fp32): grad_src (contiguous [shape]) = grad_out gathered through the index (SUM), divided by the slot's
+ * count (MEAN, counts read from the forward's scratch, fwd_scratch), or at the argmax positions only, zero elsewhere
+ * (MAX).  MEAN also writes grad_out / count to grad_out_mean (contiguous [out shape]) when it is not NULL. */
+#define GS_B200_SCATTER_MAX_DIMS 8
+enum { GS_B200_SCATTER_SUM = 0, GS_B200_SCATTER_MEAN = 1, GS_B200_SCATTER_MAX = 2 };
+enum { GS_B200_SCATTER_F32 = 0, GS_B200_SCATTER_I32 = 1, GS_B200_SCATTER_I64 = 2 };
+int32_t gs_b200_scatter_index_range(int32_t ndim, const int64_t* shape_host, int32_t dim, const int64_t* index,
+                                    const int64_t* index_strides_host, int64_t* range_out, void* stream);
+size_t gs_b200_scatter_scratch_bytes(int32_t op, int32_t dtype, int32_t ndim, const int64_t* shape_host, int32_t dim,
+                                     const int64_t* index_strides_host, int64_t dim_size);
+int32_t gs_b200_scatter_forward(int32_t op, int32_t dtype, int32_t ndim, const int64_t* shape_host, int32_t dim,
+                                int64_t dim_size, const void* src, const int64_t* src_strides_host, const int64_t* index,
+                                const int64_t* index_strides_host, void* out, const int64_t* out_strides_host,
+                                int32_t has_out, int64_t* argmax, void* scratch, void* stream);
+int32_t gs_b200_scatter_backward(int32_t op, int32_t ndim, const int64_t* shape_host, int32_t dim, int64_t dim_size,
+                                 const int64_t* index, const int64_t* index_strides_host, const float* grad_out,
+                                 const int64_t* grad_out_strides_host, const int64_t* argmax, const void* fwd_scratch,
+                                 float* grad_src, float* grad_out_mean, void* stream);
+
 /* Multi-view optimisation step with DEVICE-resident buffers: V x (forward + backward), gradients
  * summed over views into `grads` (zeroed first), packed as
  *   means3D[N,3] | shs[N,M,3] | opacities[N] | scales[N,3] | rotations[N,4] | means2D[N,3]
