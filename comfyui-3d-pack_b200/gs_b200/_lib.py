@@ -166,6 +166,16 @@ lib.ngp_b200_flexicubes_backward_attrs_workspace_bytes.argtypes = [_U4, _I, _I]
 lib.ngp_b200_flexicubes_backward_attrs.restype = _I
 lib.ngp_b200_flexicubes_backward_attrs.argtypes = [_P, _P, _P, _L, _P, _L, _P, _L, _I, _I, _I, _D, _I, _U4] + \
     [_P] * 8 + [_P, _L, _I] + [_P] * 6
+lib.ngp_b200_dmc_scratch_bytes.restype = C.c_size_t
+lib.ngp_b200_dmc_scratch_bytes.argtypes = [_I, _I, _I]
+lib.ngp_b200_dmc_count.restype = _I
+lib.ngp_b200_dmc_count.argtypes = [_P, _I, _I, _I, _F, _P, _P, _P]
+lib.ngp_b200_dmc_write.restype = _I
+lib.ngp_b200_dmc_write.argtypes = [_P, _P, _I, _I, _I, _F, _I, _I, _U4, _P, _P, _P, _P]
+lib.ngp_b200_dmc_backward_workspace_bytes.restype = C.c_size_t
+lib.ngp_b200_dmc_backward_workspace_bytes.argtypes = [_I, _I, _I]
+lib.ngp_b200_dmc_backward.restype = _I
+lib.ngp_b200_dmc_backward.argtypes = [_P, _P, _I, _I, _I, _F, _I, _U4, _P, _P, _P, _P, _P, _P]
 NGP_EXPORTS = ["ngp_b200_mlp2_supported", "ngp_b200_mlp2_fwd", "ngp_b200_mlp2_bwd","ngp_b200_grid_encode_fwd", "ngp_b200_grid_encode_bwd", "ngp_b200_grid_tv_grad", "ngp_b200_march_scratch_bytes",
                "ngp_b200_march_count", "ngp_b200_march_write", "ngp_b200_ray_ranges", "ngp_b200_weights_fwd",
                "ngp_b200_weights_bwd", "ngp_b200_accumulate_fwd", "ngp_b200_accumulate_bwd",
@@ -173,7 +183,8 @@ NGP_EXPORTS = ["ngp_b200_mlp2_supported", "ngp_b200_mlp2_fwd", "ngp_b200_mlp2_bw
                "ngp_b200_flexicubes_scratch_bytes", "ngp_b200_flexicubes_count", "ngp_b200_flexicubes_write",
                "ngp_b200_flexicubes_backward_workspace_bytes", "ngp_b200_flexicubes_backward",
                "ngp_b200_flexicubes_write_attrs", "ngp_b200_flexicubes_backward_attrs_workspace_bytes",
-               "ngp_b200_flexicubes_backward_attrs"]
+               "ngp_b200_flexicubes_backward_attrs", "ngp_b200_dmc_scratch_bytes", "ngp_b200_dmc_count",
+               "ngp_b200_dmc_write", "ngp_b200_dmc_backward_workspace_bytes", "ngp_b200_dmc_backward"]
 
 lib.gs_b200_activate.restype = _I
 lib.gs_b200_activate.argtypes = [_I, _P, _P, _P, _P, _P, _P, _P]

@@ -5,7 +5,8 @@
 csrc/mc_table.cuh, written by scripts/gen_mc_table.py.  `FlexiCubes` replaces the FlexiCubes class of the FlexiCubes
 node, CRM and InstantMesh; its case table is csrc/fc_table.cuh, written by scripts/gen_fc_table.py.
 `TrellisFlexiCubes` replaces the FlexiCubes of TRELLIS and Stable3DGen's mesh decoders (cube2mesh.py), the same
-extraction with per-vertex colours.  No CPU path."""
+extraction with per-vertex colours.  `DiffDMC` replaces diso's differentiable dual marching cubes, the mesh
+extraction of TripoSG and Hunyuan3D (FlashVDM); it shares FlexiCubes' case table.  No CPU path."""
 import ctypes as C
 
 import torch
@@ -269,3 +270,85 @@ class TrellisFlexiCubes:
         s = scalar_field.float().contiguous()
         return _FlexiCubesFn.apply(x, s, beta, alpha, gamma_f, voxelgrid_colors, R, float(weight_scale),
                                    bool(training))
+
+
+# ---- dual marching cubes (diso.DiffDMC) ----------------------------------------------------------------------------
+class _DiffDMCFn(torch.autograd.Function):
+    """Dual marching cubes through ngp_b200_dmc_{count,write,backward}; returns (verts, faces)."""
+    @staticmethod
+    def forward(ctx, grid, deform, iso, return_quads, normalize):
+        dev = grid.device
+        X, Y, Z = grid.shape
+        opt = lambda t: _P(t) if t is not None else None
+        with torch.cuda.device(dev):
+            stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+            scratch = torch.empty(int(_lib.lib.ngp_b200_dmc_scratch_bytes(X, Y, Z)), dtype=torch.uint8, device=dev)
+            totals = torch.empty(3, dtype=torch.int64, device=dev)
+            _lib.check(_lib.lib.ngp_b200_dmc_count(_P(grid), X, Y, Z, iso, _P(totals), _P(scratch), stream))
+            nv, nq, flags = totals.tolist()                     # the one host read
+            host = (C.c_ulonglong * 3)(nv, nq, flags)
+            ok = max(nv, nq) < 2 ** 31                          # otherwise the write call fails with the library's message
+            verts = torch.empty((nv if ok else 0, 3), dtype=torch.float32, device=dev)
+            shape = (nq, 4) if return_quads else (2 * nq, 3)
+            faces = torch.empty(shape if ok else (0, shape[1]), dtype=torch.int32, device=dev)
+            _lib.check(_lib.lib.ngp_b200_dmc_write(_P(grid), opt(deform), X, Y, Z, iso, int(return_quads),
+                                                   int(normalize), host, _P(verts), _P(faces), _P(scratch), stream))
+        ctx.mark_non_differentiable(faces)
+        ctx.save_for_backward(grid, deform, scratch)
+        ctx.meta = (iso, normalize, (nv, nq, flags))
+        return verts, faces
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, gverts, _gfaces):
+        grid, deform, scratch = ctx.saved_tensors
+        iso, normalize, totals = ctx.meta
+        need = ctx.needs_input_grad
+        dev = grid.device
+        X, Y, Z = grid.shape
+        gverts = torch.zeros((totals[0], 3), dtype=torch.float32, device=dev) if gverts is None \
+            else gverts.float().contiguous()
+        gg = torch.empty_like(grid) if need[0] else None
+        gd = torch.empty_like(deform) if deform is not None and need[1] else None
+        opt = lambda t: _P(t) if t is not None else None
+        with torch.cuda.device(dev):
+            stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+            work = torch.empty(max(int(_lib.lib.ngp_b200_dmc_backward_workspace_bytes(X, Y, Z)), 1), dtype=torch.uint8,
+                               device=dev)
+            _lib.check(_lib.lib.ngp_b200_dmc_backward(_P(grid), opt(deform), X, Y, Z, iso, int(normalize),
+                                                      (C.c_ulonglong * 3)(*totals), _P(gverts), opt(gg), opt(gd),
+                                                      _P(scratch), _P(work), stream))
+        return gg, gd, None, None, None
+
+
+class DiffDMC(torch.nn.Module):
+    """Differentiable dual marching cubes on the GPU (the sm_90a kernels behind ngp_b200_dmc_*): a drop-in for
+    diso.DiffDMC as TripoSG (inference_utils.py:466-472) and Hunyuan3D's DMCSurfaceExtractor call it.  The contract
+    is include/ngp_b200.h's: the grid is closed by a virtual ring of samples isovalue + 1, cubes with a non-finite
+    corner are masked, vertices and faces come in a fixed order, and gradients are bit-identical from run to run.
+    Parity with diso's own binaries is unpinned.  fp32 only; no parameters, so .to(device) is a no-op.  No CPU path."""
+
+    def __init__(self, dtype=torch.float32):
+        super().__init__()
+        if dtype != torch.float32:
+            raise NotImplementedError(f"DiffDMC: only dtype=torch.float32 is implemented on the GPU path, got {dtype}")
+        self.dtype = dtype
+
+    def forward(self, grid, deform=None, isovalue=0.0, return_quads=False, normalize=True):
+        """(vertices fp32 [V,3], faces int32 [2Q,3], or quads int32 [Q,4] with return_quads) on the grid's device,
+        computed on the current stream with one host read; differentiable in grid and deform."""
+        if not isinstance(grid, torch.Tensor) or not grid.is_cuda or grid.dtype != torch.float32:
+            raise TypeError("DiffDMC: grid must be a CUDA float32 tensor (gs_b200 has no CPU path), got "
+                            f"{getattr(grid, 'dtype', type(grid))} on {getattr(grid, 'device', None)}")
+        if grid.dim() != 3 or grid.numel() == 0:
+            raise ValueError(f"DiffDMC: grid must be a non-empty 3-D [X,Y,Z] tensor, got shape {tuple(grid.shape)}")
+        if normalize and min(grid.shape) < 2:
+            raise ValueError(f"DiffDMC: normalize divides by (dim - 1), so every dimension must be >= 2, got "
+                             f"{tuple(grid.shape)}")
+        if deform is not None:
+            if not isinstance(deform, torch.Tensor) or deform.device != grid.device or deform.dtype != torch.float32:
+                raise TypeError("DiffDMC: deform must be a float32 tensor on the grid's device")
+            if tuple(deform.shape) != (*grid.shape, 3):
+                raise ValueError(f"DiffDMC: deform must have shape {(*grid.shape, 3)}, got {tuple(deform.shape)}")
+            deform = deform.contiguous()
+        return _DiffDMCFn.apply(grid.contiguous(), deform, float(isovalue), bool(return_quads), bool(normalize))

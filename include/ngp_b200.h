@@ -133,6 +133,38 @@ int32_t ngp_b200_flexicubes_backward_attrs(const float* x, const float* s, const
                                            const float* attrs, int64_t attr_row_stride, int32_t C,
                                            const float* vattrs, const float* grad_vattrs, float* grad_attrs,
                                            void* scratch, void* workspace, void* stream);
+/* ---- differentiable dual marching cubes (the diso.DiffDMC contract of TripoSG inference_utils.py:466-472 and
+ * Hunyuan3D's DMCSurfaceExtractor; parity with diso's binaries is unpinned) -------------------------------------------
+ * grid[X,Y,Z] fp32 C-contiguous; deform[X,Y,Z,3] fp32 in index units, or NULL for none.  The grid is read as if
+ * padded by a ring of samples iso + 1 with deform 0 (no copy is made), which closes surfaces cut by the border.
+ * Point (i,j,k) sits at (i,j,k) + deform[i,j,k]; a sample is below iff value < iso in fp32.  A cube with a non-finite
+ * corner is masked: no vertex, and no quad uses it.  An unmasked cube's case is fc_table.cuh's (bit c = corner c
+ * below) and its dual vertices are its fc_group_of groups, with no ambiguity swap.  A crossed edge is crossed from
+ * its lower end a: p_a + t (p_b - p_a), t = (iso - s_a) / (s_b - s_a); a vertex is the fp32 mean of its group's
+ * crossings in ascending edge order, in unpadded index units, column c divided by dim_c - 1 if `normalize`.  One quad
+ * per crossed edge whose 4 cubes are unmasked, starting at the lowest cube, with its right-hand normal pointing from
+ * the edge's above end to its below end.  Triangles (quads == 0): (0,1,3),(1,2,3) iff the larger corner cosine of
+ * that pair is strictly below that of (0,1,2),(0,2,3), cosines taken on the output vertices.
+ * Order: vertices by (padded cube, group), quads by (lower padded point, axis), two triangles per quad in quad order.
+ * count -> (host copies totals_dev3) -> write.  totals = {vertices V, quads Q, flags}: flags bit 0/1/2 = some sample
+ * is below / above (> iso) / NaN; V = Q = 0 when no sample is NaN and none is below or none above.  write fails,
+ * before writing anything, when V or Q reaches 2^31, and with normalize on a dimension < 2.  verts[V,3] fp32,
+ * faces[Q,4] or [2Q,3] int32.  backward needs no host read and no workspace (workspace_bytes is 0): grad_verts[V,3]
+ * in; grad_grid[X,Y,Z] and grad_deform[X,Y,Z,3] (NULL = not wanted) written in full, each point gathering its up to
+ * 6 crossed edges, each edge summing dL/dv / n_group over its unmasked cubes, in fixed order (bit-identical from run
+ * to run).  Z <= 3000.  scratch >= dmc_scratch_bytes (~4.3 MB at 513^3) is passed unchanged from count to write to
+ * backward. */
+size_t ngp_b200_dmc_scratch_bytes(int32_t X, int32_t Y, int32_t Z);
+int32_t ngp_b200_dmc_count(const float* grid, int32_t X, int32_t Y, int32_t Z, float iso,
+                           unsigned long long* totals_dev3, void* scratch, void* stream);
+int32_t ngp_b200_dmc_write(const float* grid, const float* deform, int32_t X, int32_t Y, int32_t Z, float iso,
+                           int32_t quads, int32_t normalize, const unsigned long long* totals_host3, float* verts,
+                           int32_t* faces, const void* scratch, void* stream);
+size_t ngp_b200_dmc_backward_workspace_bytes(int32_t X, int32_t Y, int32_t Z);
+int32_t ngp_b200_dmc_backward(const float* grid, const float* deform, int32_t X, int32_t Y, int32_t Z, float iso,
+                              int32_t normalize, const unsigned long long* totals_host3, const float* grad_verts,
+                              float* grad_grid, float* grad_deform, const void* scratch, void* workspace,
+                              void* stream);
 #ifdef __cplusplus
 }
 #endif
