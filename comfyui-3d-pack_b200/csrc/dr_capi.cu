@@ -13,6 +13,10 @@ size_t dr_topology_scratch_bytes(int F);
 int dr_launch_edge_opposites(const int32_t*, int, int, int32_t*, void*, cudaStream_t);
 int dr_launch_antialias_fwd(const float*, const float*, const float*, const int32_t*, const int32_t*, int, int, int, int, int, int, float*, cudaStream_t);
 int dr_launch_antialias_bwd(const float*, const float*, const float*, const int32_t*, const int32_t*, int, int, int, int, int, int, const float*, float*, float*, cudaStream_t);
+size_t cr_scratch_bytes(int F, int H, int W);
+int cr_launch_rasterize(const float*, int, const int32_t*, int, const float*, int, int, float, int32_t*, float*, void*, cudaStream_t);
+int cr_launch_interpolate(const float*, int, int, const void*, int, const float*, const void*, int, int, int, const float*, float*,
+                          float*, float*, long long*, cudaStream_t);
 
 #define DR_REQ(cond, msg) do { if (!(cond)) { gs_set_error("%s: %s", __func__, msg); return 1; } } while (0)
 
@@ -75,5 +79,37 @@ int32_t dr_b200_antialias_bwd(const float* color, const float* rast, const float
                               float* dL_dcolor, float* dL_dpos, void* stream) {
     DR_REQ(color && rast && dL_dout && dL_dcolor && (F == 0 || (pos && tri && opp && dL_dpos)), "NULL pointer");
     return dr_launch_antialias_bwd(color, rast, pos, tri, opp, B, V, F, H, W, C, dL_dout, dL_dcolor, dL_dpos, (cudaStream_t)stream);
+}
+
+size_t dr_b200_cr_scratch_bytes(int32_t F, int32_t H, int32_t W) {
+    return (F < 0 || H <= 0 || W <= 0) ? 0 : cr_scratch_bytes(F, H, W);
+}
+int32_t dr_b200_cr_rasterize(const float* pos, int32_t V, const int32_t* tri, int32_t F, const float* depth_prior, int32_t H,
+                             int32_t W, float occlusion_truncation, int32_t* findices, float* barycentric, void* scratch,
+                             void* stream) {
+    DR_REQ(V >= 0 && F >= 0 && H > 0 && W > 0, "bad sizes");
+    DR_REQ(H <= (1 << 24) && W <= (1 << 24) && (int64_t)H * W <= INT32_MAX / 3, "image too large");
+    DR_REQ(findices && barycentric && scratch && (F == 0 || (pos && tri)), "NULL pointer");
+    DR_REQ(((size_t)pos & 15) == 0, "pos must be 16-byte aligned");
+    return cr_launch_rasterize(pos, V, tri, F, depth_prior, H, W, occlusion_truncation, findices, barycentric, scratch,
+                               (cudaStream_t)stream);
+}
+int32_t dr_b200_cr_interpolate_fwd(const float* col, int32_t V, int32_t C, const void* findices, int32_t findices_f32,
+                                   const float* barycentric, const void* tri, int32_t tri_i64, int32_t F, int32_t npix,
+                                   float* out, void* stream) {
+    DR_REQ(V >= 0 && C > 0 && F >= 0 && npix >= 0 && (int64_t)npix * 3 <= INT32_MAX, "bad sizes");
+    DR_REQ(npix == 0 || (findices && barycentric && out && (F == 0 || tri) && (V == 0 || col)), "NULL pointer");
+    return cr_launch_interpolate(col, V, C, findices, findices_f32, barycentric, tri, tri_i64, F, npix, nullptr, out, nullptr,
+                                 nullptr, nullptr, (cudaStream_t)stream);
+}
+int32_t dr_b200_cr_interpolate_bwd(const float* col, int32_t V, int32_t C, const void* findices, int32_t findices_f32,
+                                   const float* barycentric, const void* tri, int32_t tri_i64, int32_t F, int32_t npix,
+                                   const float* grad_out, float* grad_barycentric, float* contrib, int64_t* contrib_index,
+                                   void* stream) {
+    DR_REQ(V >= 0 && C > 0 && F >= 0 && npix >= 0 && (int64_t)npix * 3 <= INT32_MAX, "bad sizes");
+    DR_REQ(npix == 0 || (findices && barycentric && grad_out && (F == 0 || tri) && (V == 0 || col)), "NULL pointer");
+    DR_REQ((contrib == nullptr) == (contrib_index == nullptr), "contrib and contrib_index go together");
+    return cr_launch_interpolate(col, V, C, findices, findices_f32, barycentric, tri, tri_i64, F, npix, grad_out, nullptr,
+                                 grad_barycentric, contrib, (long long*)contrib_index, (cudaStream_t)stream);
 }
 }

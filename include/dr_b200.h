@@ -60,6 +60,30 @@ int32_t dr_b200_antialias_fwd(const float* color, const float* rast, const float
 int32_t dr_b200_antialias_bwd(const float* color, const float* rast, const float* pos, const int32_t* tri,
                               const int32_t* opp, int32_t B, int32_t V, int32_t F, int32_t H, int32_t W, int32_t C,
                               const float* dL_dout, float* dL_dcolor, float* dL_dpos, void* stream);
+
+/* ---- Hunyuan3D's texture-bake rasterizer (the `custom_rasterizer` package; INTEGRATION §3) ----------------------
+ * pos[V,4] clip space; tri[F,3]; findices[H,W] int32 = face id + 1 (0 = empty); barycentric[H,W,3], perspective
+ * corrected.  Bit-identical to the reference's CPU path (csrc/cr_raster.cu states the arithmetic).  depth_prior[H,W]
+ * may be NULL (no prior); with it a pixel is skipped where depth < depth_prior*0.49999 + 0.5 + occlusion_truncation.
+ * scratch: dr_b200_cr_scratch_bytes(F, H, W) (an 8 B/pixel z-buffer and two face queues); 0 on bad sizes.
+ * H, W <= 2^24 and H*W*3 < 2^31. */
+size_t dr_b200_cr_scratch_bytes(int32_t F, int32_t H, int32_t W);
+int32_t dr_b200_cr_rasterize(const float* pos, int32_t V, const int32_t* tri, int32_t F, const float* depth_prior,
+                             int32_t H, int32_t W, float occlusion_truncation, int32_t* findices, float* barycentric,
+                             void* scratch, void* stream);
+/* out[npix,C] = ((+0 + b0 col[v0]) + b1 col[v1]) + b2 col[v2] in fp32 (torch's CPU order), for the face findices - 1 + (findices == 0) (torch's
+ * wrap of negative indices; a pixel whose face or vertex is out of range gives 0).  findices is int32, or fp32 when
+ * findices_f32; tri is int32, or int64 when tri_i64; col[V,C]. */
+int32_t dr_b200_cr_interpolate_fwd(const float* col, int32_t V, int32_t C, const void* findices, int32_t findices_f32,
+                                   const float* barycentric, const void* tri, int32_t tri_i64, int32_t F,
+                                   int32_t npix, float* out, void* stream);
+/* grad_barycentric[npix,3] (may be NULL) = sum over c in ascending order of grad_out * col[v_k];
+ * contrib[3*npix,C] = b_k * grad_out and contrib_index[3*npix] = v_k (both NULL or neither): the rows a deterministic
+ * scatter sum (gs_b200_scatter_*) folds into the col gradient.  No atomics. */
+int32_t dr_b200_cr_interpolate_bwd(const float* col, int32_t V, int32_t C, const void* findices, int32_t findices_f32,
+                                   const float* barycentric, const void* tri, int32_t tri_i64, int32_t F,
+                                   int32_t npix, const float* grad_out, float* grad_barycentric, float* contrib,
+                                   int64_t* contrib_index, void* stream);
 #ifdef __cplusplus
 }
 #endif

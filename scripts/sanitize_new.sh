@@ -36,3 +36,28 @@ torch.cuda.synchronize()
 PY
 timeout 1200 compute-sanitizer --tool memcheck --error-exitcode 9 --launch-timeout 0 python /tmp/new_case.py 2>&1 | tail -12
 echo "memcheck rc=$?"
+
+# Hunyuan3D's texture-bake rasterizer (cr_raster.cu): every queue of cr_large_kernel (thread, warp, CTA split and
+# whole-face CTA), the depth prior, interpolate forward + backward; memcheck and racecheck
+cat > /tmp/cr_case.py <<'PY'
+import sys, os
+ROOT = os.getcwd(); sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "comfyui-3d-pack_b200")); sys.path.insert(0, os.path.join(ROOT, "tests"))
+import torch
+import custom_rasterizer as cr
+from test_gpu_custom_rasterizer import large_faces, screen_filling, sphere, view_pos
+dev = torch.device("cuda:0")
+xyz, tri, _ = sphere(2000, seed=1)
+fi, b = cr.rasterize(view_pos(xyz, (96, 80)).to(dev)[None], tri.to(dev), (96, 80))
+pos, t = screen_filling()
+cr.rasterize(pos.to(dev)[None], t.to(dev), (128, 128), torch.rand(128, 128, device=dev) * 2 - 1, 1)
+pos, t, hw = large_faces(1800, (192, 256), 10)
+cr.rasterize(pos.to(dev)[None], t.to(dev), hw)
+col = torch.randn(1, xyz.shape[0], 3, device=dev, requires_grad=True)
+bq = b.clone().requires_grad_(True)
+cr.interpolate(col, fi.float(), bq, tri.to(dev)).sum().backward()
+torch.cuda.synchronize(); print("cr ok", int((fi != 0).sum()), float(col.grad.abs().sum()))
+PY
+for tool in memcheck racecheck; do
+  timeout 1200 compute-sanitizer --tool $tool --error-exitcode 9 --launch-timeout 0 python /tmp/cr_case.py 2>&1 | tail -6
+  echo "cr $tool rc=$?"
+done
