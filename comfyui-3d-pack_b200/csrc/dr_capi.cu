@@ -17,6 +17,9 @@ size_t cr_scratch_bytes(int F, int H, int W);
 int cr_launch_rasterize(const float*, int, const int32_t*, int, const float*, int, int, float, int32_t*, float*, void*, cudaStream_t);
 int cr_launch_interpolate(const float*, int, int, const void*, int, const float*, const void*, int, int, int, const float*, float*,
                           float*, float*, long long*, cudaStream_t);
+size_t ub_scratch_bytes(int F, int res);
+int ub_launch_rasterize(const float*, int, const int32_t*, int, float*, int, int, int, void*, cudaStream_t);
+int ub_launch_interpolate(const float*, int, const int32_t*, int, const float*, float*, int, int, int, cudaStream_t);
 
 #define DR_REQ(cond, msg) do { if (!(cond)) { gs_set_error("%s: %s", __func__, msg); return 1; } } while (0)
 
@@ -111,5 +114,25 @@ int32_t dr_b200_cr_interpolate_bwd(const float* col, int32_t V, int32_t C, const
     DR_REQ((contrib == nullptr) == (contrib_index == nullptr), "contrib and contrib_index go together");
     return cr_launch_interpolate(col, V, C, findices, findices_f32, barycentric, tri, tri_i64, F, npix, grad_out, nullptr,
                                  grad_barycentric, contrib, (long long*)contrib_index, (cudaStream_t)stream);
+}
+
+size_t dr_b200_uvbake_scratch_bytes(int32_t F, int32_t res) {
+    return (F < 0 || res <= 0 || res > (1 << 15)) ? 0 : ub_scratch_bytes(F, res);
+}
+int32_t dr_b200_uvbake_rasterize(const float* uv, int32_t V, const int32_t* faces, int32_t F, float* out, int32_t res,
+                                 int32_t rows, int32_t cols, void* scratch, void* stream) {
+    DR_REQ(V >= 0 && F >= 0 && res > 0 && res <= (1 << 15) && rows >= 0 && cols >= 0, "bad sizes");
+    DR_REQ(out && scratch && (F == 0 || (uv && faces)), "NULL pointer");
+    DR_REQ(((size_t)uv & 7) == 0 && ((size_t)out & 15) == 0, "uv must be 8-byte and out 16-byte aligned");
+    return ub_launch_rasterize(uv, V, faces, F, out, res, rows < res ? rows : res, cols < res ? cols : res, scratch,
+                               (cudaStream_t)stream);
+}
+int32_t dr_b200_uvbake_interpolate(const float* attr, int32_t V, const int32_t* faces, int32_t F, const float* rast,
+                                   float* out, int32_t res, int32_t rows, int32_t cols, void* stream) {
+    DR_REQ(V >= 0 && F >= 0 && res > 0 && res <= (1 << 15) && rows >= 0 && cols >= 0, "bad sizes");
+    DR_REQ(rast && out && (F == 0 || faces) && (V == 0 || attr), "NULL pointer");
+    DR_REQ(((size_t)rast & 15) == 0, "rast must be 16-byte aligned");
+    return ub_launch_interpolate(attr, V, faces, F, rast, out, res, rows < res ? rows : res, cols < res ? cols : res,
+                                 (cudaStream_t)stream);
 }
 }

@@ -113,6 +113,13 @@ lib.dr_b200_cr_interpolate_fwd.restype = _I
 lib.dr_b200_cr_interpolate_fwd.argtypes = [_P, _I, _I, _P, _I, _P, _P, _I, _I, _I, _P, _P]
 lib.dr_b200_cr_interpolate_bwd.restype = _I
 lib.dr_b200_cr_interpolate_bwd.argtypes = [_P, _I, _I, _P, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P]
+lib.dr_b200_uvbake_scratch_bytes.restype = C.c_size_t
+lib.dr_b200_uvbake_scratch_bytes.argtypes = [_I, _I]
+lib.dr_b200_uvbake_rasterize.restype = _I
+lib.dr_b200_uvbake_rasterize.argtypes = [_P, _I, _P, _I, _P, _I, _I, _I, _P, _P]
+lib.dr_b200_uvbake_interpolate.restype = _I
+lib.dr_b200_uvbake_interpolate.argtypes = [_P, _I, _P, _I, _P, _P, _I, _I, _I, _P]
+UVBAKE_EXPORTS = ["dr_b200_uvbake_scratch_bytes", "dr_b200_uvbake_rasterize", "dr_b200_uvbake_interpolate"]
 CR_EXPORTS = ["dr_b200_cr_scratch_bytes", "dr_b200_cr_rasterize", "dr_b200_cr_interpolate_fwd", "dr_b200_cr_interpolate_bwd"]
 DR_EXPORTS = ["dr_b200_rasterize_scratch_bytes", "dr_b200_rasterize_fwd", "dr_b200_rasterize_bwd",
               "dr_b200_interpolate_fwd", "dr_b200_interpolate_bwd", "dr_b200_texture_fwd", "dr_b200_texture_bwd",
@@ -241,7 +248,8 @@ lib.gs_b200_composite_bwd_occupancy.argtypes = [C.POINTER(C.c_int32), C.POINTER(
 EXPORTS = ["gs_b200_set_grad_sink", "gs_b200_composite_bwd_occupancy", "gs_b200_image_loss", "gs_b200_step_device_train", "gs_b200_step_device_hook", "gs_b200_render_views", "gs_b200_set_tile_culling", "gs_b200_get_tile_culling", "gs_b200_step_device", "gs_b200_step_host_dev_grads", "gs_b200_launch_count", "gs_b200_profile_enable", "gs_b200_profile_read",
            "gs_b200_abi_version", "gs_b200_last_error", "gs_b200_rasterize_forward", "gs_b200_rasterize_backward",
            "gs_b200_state_free", "gs_b200_debug_sorted_keys", "gs_b200_sort_scratch_bytes",
-           "gs_b200_sort_pairs_u32", "gs_b200_knn_mean_dist2", "gs_b200_step_host"] + SCATTER_EXPORTS + CR_EXPORTS
+           "gs_b200_sort_pairs_u32", "gs_b200_knn_mean_dist2", "gs_b200_step_host"] + SCATTER_EXPORTS + CR_EXPORTS + \
+    UVBAKE_EXPORTS
 
 
 def last_error() -> str:

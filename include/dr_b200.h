@@ -84,6 +84,22 @@ int32_t dr_b200_cr_interpolate_bwd(const float* col, int32_t V, int32_t C, const
                                    const float* barycentric, const void* tri, int32_t tri_i64, int32_t F,
                                    int32_t npix, const float* grad_out, float* grad_barycentric, float* contrib,
                                    int64_t* contrib_index, void* stream);
+
+/* ---- StableFast3D's UV texture baker (slangtorch's texture_baker.slang: bake_uv, interpolate; INTEGRATION §3) ------
+ * Bit-identical to the reference's own kernels (csrc/uv_bake.cu states the arithmetic).  uv[V,2] fp32 (8-byte
+ * aligned), faces[F,3] int32, square textures of res x res texels, res <= 2^15.  Only the launched region, texel rows
+ * [0, rows) and columns [0, cols) (clipped to res), is written; the rest of out keeps what it held.
+ * rasterize: out[res,res,4] (16-byte aligned) = (u, v, w, face) of the lowest-index face whose barycentric test
+ * accepts the texel, or (0, 0, 0, -1).  A face with a vertex id out of range is skipped.
+ * scratch: dr_b200_uvbake_scratch_bytes(F, res) = 256 + 4 res^2 + 8 F bytes; 0 on bad sizes.  After a call its first
+ * three uint32 hold the warp-queue, CTA-queue and whole-texture face counts (whole-texture faces are in the CTA queue).
+ * interpolate: out[res,res,3] = the rast-weighted attr[V,3] of face (int)rast.w, 0 where that id is negative or any
+ * face or vertex id is out of range; rast[res,res,4] 16-byte aligned. */
+size_t dr_b200_uvbake_scratch_bytes(int32_t F, int32_t res);
+int32_t dr_b200_uvbake_rasterize(const float* uv, int32_t V, const int32_t* faces, int32_t F, float* out, int32_t res,
+                                 int32_t rows, int32_t cols, void* scratch, void* stream);
+int32_t dr_b200_uvbake_interpolate(const float* attr, int32_t V, const int32_t* faces, int32_t F, const float* rast,
+                                   float* out, int32_t res, int32_t rows, int32_t cols, void* stream);
 #ifdef __cplusplus
 }
 #endif

@@ -61,3 +61,25 @@ for tool in memcheck racecheck; do
   timeout 1200 compute-sanitizer --tool $tool --error-exitcode 9 --launch-timeout 0 python /tmp/cr_case.py 2>&1 | tail -6
   echo "cr $tool rc=$?"
 done
+
+# StableFast3D's texture baker (uv_bake.cu): every queue (thread, warp, CTA split, CTA whole-face, whole-texture), a
+# region with res % 16 != 0, and interpolate with out-of-range ids; memcheck and racecheck
+cat > /tmp/ub_case.py <<'PY'
+import sys, os
+ROOT = os.getcwd(); sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "comfyui-3d-pack_b200"))
+import numpy as np, torch
+from gs_b200 import uv_bake
+from oracle import uvbake_oracle as O
+dev = torch.device("cuda:0")
+t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+for name, (uv, faces, res) in {**O.queue_cases(0), "nonfinite": O.adversarial(0)["nonfinite"]}.items():
+    out = torch.zeros(res, res, 4, device=dev)
+    uv_bake.rasterize_into(t(uv), t(faces), out, res - 5, res - 9)
+    bad = faces.copy(); bad[::5, 1] = -3
+    uv_bake.interpolate_into(t(np.random.rand(uv.shape[0], 3).astype(np.float32)), out, t(bad), torch.zeros(res, res, 3, device=dev), res, res)
+torch.cuda.synchronize(); print("ub ok")
+PY
+for tool in memcheck racecheck; do
+  timeout 1200 compute-sanitizer --tool $tool --error-exitcode 9 --launch-timeout 0 python /tmp/ub_case.py 2>&1 | tail -6
+  echo "ub $tool rc=$?"
+done
