@@ -9,7 +9,7 @@
 //   * 1/(det^2 + 1e-7) in the conic->cov2D chain;
 //   * zero gradient to t.x / t.y when the 1.3*tanfov clamp is active, while
 //     t.z differentiates J with the clamped value held fixed;
-//   * SH clamp mask; quaternion NOT normalised inside.
+//   * SH clamp mask, decided on the forward's own colour (gs_sh_colour); quaternion NOT normalised inside.
 //
 // Two kernels share one per-view device function:
 //   preprocess_backward_kernel        one view  (the drop-in backward op)
@@ -104,6 +104,9 @@ __device__ __forceinline__ void backward_view(const ViewB& vb, int M, float x, f
     if (has_sh) {
         const int deg = vb.deg;
         const float vx = x - vb.cam[0], vy = y - vb.cam[1], vz = z - vb.cam[2];
+        // the clamp mask is decided on the forward's colour, bit for bit (the chain below keeps its own arithmetic)
+        float rgb[3];
+        gs_sh_colour(deg, sh_row, vx, vy, vz, rgb);
         const float inv = 1.0f / sqrtf(vx * vx + vy * vy + vz * vz);
         const float dx = vx * inv, dy = vy * inv, dz = vz * inv;
         float bas[16], bx[16], by[16], bz[16];
@@ -136,11 +139,7 @@ __device__ __forceinline__ void backward_view(const ViewB& vb, int M, float x, f
                 }
             }
         }
-        float r = 0.5f, g = 0.5f, b = 0.5f;
-#pragma unroll
-        for (int k = 0; k < 16; k++)
-            if (k < nb) { r += bas[k] * sh_row[3 * k]; g += bas[k] * sh_row[3 * k + 1]; b += bas[k] * sh_row[3 * k + 2]; }
-        const float dr = (r < 0.f) ? 0.f : gk.x, dg = (g < 0.f) ? 0.f : gk.y, db = (b < 0.f) ? 0.f : gk.z;
+        const float dr = (rgb[0] < 0.f) ? 0.f : gk.x, dg = (rgb[1] < 0.f) ? 0.f : gk.y, db = (rgb[2] < 0.f) ? 0.f : gk.z;
         float ddx = 0.f, ddy = 0.f, ddz = 0.f;
 #pragma unroll
         for (int k = 0; k < 16; k++) {
@@ -287,7 +286,7 @@ preprocess_backward_kernel(ViewArgs va, int N, int M, const float* __restrict__ 
 
 // V views in one pass (SH + scale/rotation parameterisation only — what the optimisation step uses).
 // sg, radii: [V][N].
-__global__ void __launch_bounds__(PB_THREADS, 4)     // 128 registers, no spills: 4 CTAs / SM (was 168 -> 3)
+__global__ void __launch_bounds__(PB_THREADS, 4)     // 128 registers: 4 CTAs / SM (was 168 -> 3)
 preprocess_backward_multi_kernel(const float* __restrict__ views, int V, int W, int H, int sh_degree,
                                  float scale_modifier, int N, int M, const float* __restrict__ means3D,
                                  const float* __restrict__ shs, const float* __restrict__ scales,

@@ -133,6 +133,37 @@ int check_inputs(int N, int M, int sh_degree, const float* means3D, const float*
     return 0;
 }
 
+// The multi-view step's view chunks: nchunks balanced chunks of <= VB views (VB <= 16, one batched preprocess, binning
+// and preprocess backward each); chunk k holds views [k VB, min(V, (k + 1) VB)).
+struct StepChunks {
+    int nchunks, VB;
+    explicit StepChunks(int V) {
+        const int maxv = std::min(gs_preprocess_multi_max_views(), GS_MAX_SEGS);
+        nchunks = (V + maxv - 1) / maxv;
+        VB = nchunks > 0 ? (V + nchunks - 1) / nchunks : 0;
+    }
+};
+
+// Preprocess backward of step chunk k (views [v0, v0 + nv)): the first chunk writes the gradients, later ones add to
+// them.  Run over `nparts` Gaussian ranges whose starts are multiples of the kernel's 128-Gaussian CTA; after(first,
+// count) follows each range's launch (a gradient sink starts the range's transfer there).
+template <class After>
+int step_backward_chunk(int k, int nparts, const float* views_chunk, int nv, int W, int H, int sh_degree,
+                        float scale_modifier, int N, int M, const float* means, const float* shs, const float* scales,
+                        const float* rots, const int32_t* radii, const SplatGrad* sg, float* gmeans, float* gm2d,
+                        float* gshs, float* gopac, float* gscales, float* grots, cudaStream_t s, After after) {
+    const int per = (((N + nparts - 1) / nparts) + 127) / 128 * 128;
+    for (int first = 0; first < N; first += per) {
+        const int count = std::min(per, N - first);
+        { StageTimer t(8, s);
+        if (gs_launch_preprocess_backward_multi(views_chunk, nv, W, H, sh_degree, scale_modifier, N, M, means, shs, scales,
+                                                rots, radii, sg, gmeans, gm2d, gshs, gopac, gscales, grots, k > 0 ? 1 : 0,
+                                                first, count, s)) return 1; }
+        after(first, count);
+    }
+    return 0;
+}
+
 int bits_for(int n) { int b = 0; while ((1 << b) < n) b++; return b < 1 ? 1 : b; }
 
 unsigned long long* pinned_u64() {
@@ -464,6 +495,57 @@ int32_t gs_b200_debug_sorted_keys(const gs_b200_state* state, uint64_t* keys_out
                                  state->num_rendered, keys_out, (cudaStream_t)stream_);
 }
 
+int32_t gs_b200_debug_preprocess_backward(const gs_b200_view* view, int32_t N, int32_t M, const float* means3D,
+                                          const float* shs, const float* colors_precomp, const float* opacities,
+                                          const float* scales, const float* rotations, const float* cov3D_precomp,
+                                          const int32_t* radii, const double* splat_grads, float* dL_dmeans3D,
+                                          float* dL_dmeans2D, float* dL_dshs, float* dL_dcolors, float* dL_dopacities,
+                                          float* dL_dscales, float* dL_drotations, float* dL_dcov3D, int32_t accumulate,
+                                          void* stream_) {
+    ViewArgs va;
+    if (make_view_args(view, va)) return 1;
+    if (check_inputs(N, M, view->sh_degree, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp)) return 1;
+    if (N > 0 && (!radii || !splat_grads)) { gs_set_error("debug_preprocess_backward: NULL radii/splat_grads"); return 1; }
+    return gs_launch_preprocess_backward(va, N, M, means3D, shs, colors_precomp, opacities, scales, rotations,
+                                         cov3D_precomp, radii, (const SplatGrad*)splat_grads, dL_dmeans3D, dL_dmeans2D,
+                                         dL_dshs, dL_dcolors, dL_dopacities, dL_dscales, dL_drotations, dL_dcov3D,
+                                         accumulate, (cudaStream_t)stream_);
+}
+
+int32_t gs_b200_step_view_chunks(int32_t V, int32_t* bounds) {
+    if (V <= 0 || !bounds) { gs_set_error("step_view_chunks: bad argument"); return -1; }
+    const StepChunks ch(V);
+    for (int k = 0; k < ch.nchunks; k++) bounds[k] = k * ch.VB;
+    bounds[ch.nchunks] = V;
+    return ch.nchunks;
+}
+
+// The preprocess backward of the multi-view step, as step_core runs it: the same chunks (StepChunks) and the same
+// per-chunk launches (step_backward_chunk), the last chunk over `nparts` Gaussian ranges as with a gradient sink.
+int32_t gs_b200_debug_preprocess_backward_multi(int32_t V, int32_t H, int32_t W, int32_t sh_degree, float scale_modifier,
+                                                const float* views_dev, int32_t N, int32_t M, const float* means3D,
+                                                const float* shs, const float* scales, const float* rotations,
+                                                const int32_t* radii, const double* splat_grads, float* grads_dev,
+                                                int32_t nparts, void* stream_) {
+    cudaStream_t s = (cudaStream_t)stream_;
+    if (V <= 0 || N <= 0 || M < (sh_degree + 1) * (sh_degree + 1) || M > 16 || nparts < 1 || !views_dev || !means3D ||
+        !shs || !scales || !rotations || !radii || !splat_grads || !grads_dev) {
+        gs_set_error("debug_preprocess_backward_multi: bad argument"); return 1;
+    }
+    // the step's gradient layout: means 3N | shs 3NM | opacities N | scales 3N | rotations 4N | means2D 3N
+    float* gm = grads_dev; float* gsh = gm + 3 * (size_t)N; float* gop = gsh + 3 * (size_t)N * M;
+    float* gsc = gop + N; float* grt = gsc + 3 * (size_t)N; float* g2 = grt + 4 * (size_t)N;
+    const SplatGrad* sg = (const SplatGrad*)splat_grads;
+    const StepChunks ch(V);
+    for (int k = 0; k < ch.nchunks; k++) {
+        const int v0 = k * ch.VB, nv = std::min(ch.VB, V - v0);
+        if (step_backward_chunk(k, k + 1 == ch.nchunks ? nparts : 1, views_dev + (size_t)v0 * 40, nv, W, H, sh_degree,
+                                scale_modifier, N, M, means3D, shs, scales, rotations, radii + (size_t)v0 * N,
+                                sg + (size_t)v0 * N, gm, g2, gsh, gop, gsc, grt, s, [](int, int) {})) return 1;
+    }
+    return 0;
+}
+
 int32_t gs_b200_knn_mean_dist2(const float* points, int32_t N, float* out, void* stream_) {
     return gs_launch_knn(points, N, out, (cudaStream_t)stream_);
 }
@@ -598,9 +680,8 @@ int step_core(int V, int H, int W, int sh_degree, float scale_modifier, const fl
     // pre+bin(k+1) is enqueued when chunk k's views start (its second half, after the host has read the pair counts,
     // once they have all been enqueued), bwd(k) after that; two workspace sets alternate and the aux stream's own
     // order (bwd(k-1) before pre(k+1)) protects their reuse.
-    const int maxv = std::min(gs_preprocess_multi_max_views(), GS_MAX_SEGS);
-    const int nchunks = (V + maxv - 1) / maxv;
-    const int VB = (V + nchunks - 1) / nchunks;
+    const StepChunks chunks(V);
+    const int nchunks = chunks.nchunks, VB = chunks.VB;
     const size_t nvb = (size_t)VB * N;
     const bool tight = g_tile_culling.load() >= 1;
     const bool late = O.shs_ready && par.shs && !par.colors;
@@ -734,16 +815,11 @@ int step_core(int V, int H, int W, int sh_degree, float scale_modifier, const fl
         if (O.forward_only) continue;
         const bool last_chunk = k + 1 == nchunks;
         const int nparts = (sink && last_chunk && sink->nchunks > 1) ? sink->nchunks : 1;
-        const int per = (((N + nparts - 1) / nparts) + 127) / 128 * 128;
-        for (int first = 0; first < N && !rc; first += per) {
-            const int count = std::min(per, N - first);
-            { StageTimer t(8, aux);
-            rc = gs_launch_preprocess_backward_multi(views_dev + (size_t)v0 * 40, nv, W, H, sh_degree, scale_modifier, N, M,
-                                                     par.means, par.shs, par.scales, par.rots, w.radii, w.sg, grd.means,
-                                                     grd.m2d, grd.shs, grd.opac, grd.scales, grd.rots, k > 0 ? 1 : 0, first,
-                                                     count, aux); }
-            if (!rc && sink && last_chunk) sink->fn(sink->ctx, first, count, aux);
-        }
+        rc = step_backward_chunk(k, nparts, views_dev + (size_t)v0 * 40, nv, W, H, sh_degree, scale_modifier, N, M,
+                                 par.means, par.shs, par.scales, par.rots, w.radii, w.sg, grd.means, grd.m2d, grd.shs,
+                                 grd.opac, grd.scales, grd.rots, aux, [&](int first, int count) {
+                                     if (sink && last_chunk) sink->fn(sink->ctx, first, count, aux);
+                                 });
     }
     // join: the caller's stream continues after the aux stream (which has waited for both slot streams)
     for (int i = 0; i < NSLOTS; i++) {          // (on an error path the slots may not have been joined into aux yet)

@@ -26,6 +26,43 @@
 #define SH_C3_5 1.445305721320277f
 #define SH_C3_6 -0.5900435899266435f
 
+// SH colour of one Gaussian before the max with 0, from v = mean - campos: the forward's record colour and the
+// backward's clamp mask (channel < 0 passes no gradient) both come from here, so the mask is the forward's decision
+// bit for bit.  Every operation is an explicit round-to-nearest intrinsic, so no -fmad setting of the including
+// translation unit changes a bit: one fma per basis function in order from 0, then + 0.5
+// (oracle/gs_bwd_oracle.py sh_colour32).  Each basis value is consumed as it is made, so few registers stay live.
+__device__ __forceinline__ void gs_sh_colour(int deg, const float* __restrict__ sh, float vx, float vy, float vz,
+                                             float rgb[3]) {
+    const float inv = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(vx, vx), __fmul_rn(vy, vy)), __fmul_rn(vz, vz))));
+    const float x = __fmul_rn(vx, inv), y = __fmul_rn(vy, inv), z = __fmul_rn(vz, inv);
+    float r = 0.f, g = 0.f, b = 0.f;
+    auto acc = [&](int k, float bk) {
+        r = __fmaf_rn(bk, sh[3 * k + 0], r); g = __fmaf_rn(bk, sh[3 * k + 1], g); b = __fmaf_rn(bk, sh[3 * k + 2], b);
+    };
+    acc(0, SH_C0);
+    if (deg > 0) {
+        acc(1, __fmul_rn(-SH_C1, y)); acc(2, __fmul_rn(SH_C1, z)); acc(3, __fmul_rn(-SH_C1, x));
+        if (deg > 1) {
+            const float xx = __fmul_rn(x, x), yy = __fmul_rn(y, y), zz = __fmul_rn(z, z);
+            const float xy = __fmul_rn(x, y), yz = __fmul_rn(y, z), xz = __fmul_rn(x, z);
+            acc(4, __fmul_rn(SH_C2_0, xy)); acc(5, __fmul_rn(SH_C2_1, yz));
+            acc(6, __fmul_rn(SH_C2_2, __fsub_rn(__fsub_rn(__fmul_rn(2.0f, zz), xx), yy)));
+            acc(7, __fmul_rn(SH_C2_3, xz)); acc(8, __fmul_rn(SH_C2_4, __fsub_rn(xx, yy)));
+            if (deg > 2) {
+                const float xx3 = __fmul_rn(3.0f, xx), yy3 = __fmul_rn(3.0f, yy);
+                acc(9, __fmul_rn(__fmul_rn(SH_C3_0, y), __fsub_rn(xx3, yy)));
+                acc(10, __fmul_rn(__fmul_rn(SH_C3_1, xy), z));
+                acc(11, __fmul_rn(__fmul_rn(SH_C3_2, y), __fsub_rn(__fsub_rn(__fmul_rn(4.0f, zz), xx), yy)));
+                acc(12, __fmul_rn(__fmul_rn(SH_C3_3, z), __fsub_rn(__fsub_rn(__fmul_rn(2.0f, zz), xx3), yy3)));
+                acc(13, __fmul_rn(__fmul_rn(SH_C3_4, x), __fsub_rn(__fsub_rn(__fmul_rn(4.0f, zz), xx), yy)));
+                acc(14, __fmul_rn(__fmul_rn(SH_C3_5, z), __fsub_rn(xx, yy)));
+                acc(15, __fmul_rn(__fmul_rn(SH_C3_6, x), __fsub_rn(xx, yy3)));
+            }
+        }
+    }
+    rgb[0] = __fadd_rn(r, 0.5f); rgb[1] = __fadd_rn(g, 0.5f); rgb[2] = __fadd_rn(b, 0.5f);
+}
+
 // Per-Gaussian splat record, 48 B = 3 x 128-bit, written by preprocess and
 // gathered (3 x LDG.128) by the composite kernels.
 struct __align__(16) SplatRec {

@@ -14,44 +14,12 @@
 
 namespace {
 
-__device__ __forceinline__ void sh_to_rgb(int deg, int M, const float* __restrict__ sh, float dx, float dy,
-                                          float dz, float& r, float& g, float& b) {
-    // sh: [M,3] of this Gaussian.  Basis as shared_utils/sh_utils.py:57-112.
-    float inv = 1.0f / sqrtf(dx * dx + dy * dy + dz * dz);
-    float x = dx * inv, y = dy * inv, z = dz * inv;
-    float bas[16];
-    bas[0] = SH_C0;
-    int nb = 1;
-    if (deg > 0) {
-        bas[1] = -SH_C1 * y; bas[2] = SH_C1 * z; bas[3] = -SH_C1 * x; nb = 4;
-        if (deg > 1) {
-            float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
-            bas[4] = SH_C2_0 * xy; bas[5] = SH_C2_1 * yz; bas[6] = SH_C2_2 * (2.0f * zz - xx - yy);
-            bas[7] = SH_C2_3 * xz; bas[8] = SH_C2_4 * (xx - yy); nb = 9;
-            if (deg > 2) {
-                bas[9] = SH_C3_0 * y * (3.0f * xx - yy);
-                bas[10] = SH_C3_1 * xy * z;
-                bas[11] = SH_C3_2 * y * (4.0f * zz - xx - yy);
-                bas[12] = SH_C3_3 * z * (2.0f * zz - 3.0f * xx - 3.0f * yy);
-                bas[13] = SH_C3_4 * x * (4.0f * zz - xx - yy);
-                bas[14] = SH_C3_5 * z * (xx - yy);
-                bas[15] = SH_C3_6 * x * (xx - 3.0f * yy);
-                nb = 16;
-            }
-        }
-    }
-    r = 0.f; g = 0.f; b = 0.f;
-#pragma unroll
-    for (int k = 0; k < 16; k++) {
-        if (k < nb) {
-            // explicit FMAs: this translation unit is compiled with -fmad=false for the sake of the integer outputs
-            // (radius, tile rectangle, depth key); the colour is compared to 1e-4, so the dot product may contract
-            r = fmaf(bas[k], sh[3 * k + 0], r);
-            g = fmaf(bas[k], sh[3 * k + 1], g);
-            b = fmaf(bas[k], sh[3 * k + 2], b);
-        }
-    }
-    r = fmaxf(r + 0.5f, 0.f); g = fmaxf(g + 0.5f, 0.f); b = fmaxf(b + 0.5f, 0.f);
+__device__ __forceinline__ void sh_to_rgb(int deg, const float* __restrict__ sh, float dx, float dy, float dz, float& r,
+                                          float& g, float& b) {
+    // sh: [M,3] of this Gaussian.  Basis as shared_utils/sh_utils.py:57-112; gs_sh_colour is shared with the backward
+    float rgb[3];
+    gs_sh_colour(deg, sh, dx, dy, dz, rgb);
+    r = fmaxf(rgb[0], 0.f); g = fmaxf(rgb[1], 0.f); b = fmaxf(rgb[2], 0.f);
 }
 
 constexpr int PP_THREADS = 128;
@@ -197,7 +165,7 @@ __device__ __forceinline__ void project_view(const ViewK& vk, int deg, int M, fl
     dkey = __float_as_uint(tz);
     float cr, cg, cbl;
     if (col != nullptr) { cr = col[0]; cg = col[1]; cbl = col[2]; }
-    else if (sh_row != nullptr) sh_to_rgb(deg, M, sh_row, x - vk.cam[0], y - vk.cam[1], z - vk.cam[2], cr, cg, cbl);
+    else if (sh_row != nullptr) sh_to_rgb(deg, sh_row, x - vk.cam[0], y - vk.cam[1], z - vk.cam[2], cr, cg, cbl);
     else { cr = 0.f; cg = 0.f; cbl = 0.f; }       // geometry-only pass: sh_colour_multi_kernel fills the colour in later
     rec.g = make_float4(px, py, tz, __int_as_float(rad_i));
     // conic pre-scaled to log2 units for the composite: a' = -0.5*log2e*A, b' = -log2e*B, c' = -0.5*log2e*C
@@ -334,7 +302,7 @@ sh_colour_multi_kernel(const float* __restrict__ views, int V, int sh_degree, in
         const size_t o = (size_t)v * N + idx;
         if (radii[o] <= 0) continue;
         float cr, cg, cb;
-        sh_to_rgb(sh_degree, M, s_sh + tid * rowp, x - s_cam[3 * v], y - s_cam[3 * v + 1], z - s_cam[3 * v + 2], cr, cg, cb);
+        sh_to_rgb(sh_degree, s_sh + tid * rowp, x - s_cam[3 * v], y - s_cam[3 * v + 1], z - s_cam[3 * v + 2], cr, cg, cb);
         float* k = reinterpret_cast<float*>(&recs[o].k);
         *reinterpret_cast<float2*>(k) = make_float2(cr, cg);
         k[2] = cb;

@@ -136,6 +136,28 @@ int32_t gs_b200_state_free(gs_b200_state* state, void* stream);
  * the package's binning stage would hold, for bit-exact comparison. keys_out[P]. */
 int32_t gs_b200_debug_sorted_keys(const gs_b200_state* state, uint64_t* keys_out, void* stream);
 
+/* Tests: the per-Gaussian preprocess backward alone, fed with per-splat sums the caller chooses instead of the
+ * composite's.  splat_grads: [V][N][12] double, per splat (sum w dx, sum w dy, dL/ddepth, 0, sum w dx dx,
+ * sum w dx dy, sum w dy dy, dL/dopacity, dL/dr, dL/dg, dL/db, 0) with w = dL/dG * G; radii [V][N] as the forward
+ * wrote them.  The one-view form is the backward of gs_b200_rasterize_backward (V = 1, same arguments).  The multi-view
+ * form runs the backward of the gs_b200_step_* entries through the same code they use: views_dev [V][40] and grads_dev
+ * laid out as theirs, the views in the step's chunks (gs_b200_step_view_chunks; the first chunk writes, later ones
+ * add), the last chunk over `nparts` Gaussian ranges as with a gradient sink of `nparts` chunks. */
+int32_t gs_b200_debug_preprocess_backward(
+    const gs_b200_view* view, int32_t N, int32_t M,
+    const float* means3D, const float* shs, const float* colors_precomp, const float* opacities,
+    const float* scales, const float* rotations, const float* cov3D_precomp,
+    const int32_t* radii, const double* splat_grads,
+    float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dshs, float* dL_dcolors, float* dL_dopacities,
+    float* dL_dscales, float* dL_drotations, float* dL_dcov3D, int32_t accumulate, void* stream);
+int32_t gs_b200_debug_preprocess_backward_multi(
+    int32_t V, int32_t H, int32_t W, int32_t sh_degree, float scale_modifier, const float* views_dev,
+    int32_t N, int32_t M, const float* means3D, const float* shs, const float* scales, const float* rotations,
+    const int32_t* radii, const double* splat_grads, float* grads_dev, int32_t nparts, void* stream);
+/* The view chunks of the multi-view step for V views: bounds[k] is the first view of chunk k, bounds[nchunks] = V
+ * (bounds holds at least V + 1 entries).  Returns nchunks, or -1 on a bad argument.  Host only. */
+int32_t gs_b200_step_view_chunks(int32_t V, int32_t* bounds);
+
 /* CUB-free onesweep LSD radix sort of (u32 key, u32 value) pairs on bits
  * [begin_bit,end_bit) — the replacement for cub::DeviceRadixSort::SortPairs in
  * the package's binning stage.  keys/vals are ping-pong pairs of n elements;
