@@ -246,7 +246,7 @@ struct BinA {
     uint32_t *dkeys_alt = nullptr, *ids_alt = nullptr, *offsets = nullptr;
     unsigned long long* totals = nullptr;                                 // [nv] on the device
     void *sort_scratch = nullptr, *scan_scratch = nullptr;
-    const uint32_t* sorted_ids = nullptr;                                 // [nv][N], set by bin_a
+    const uint32_t *sorted_ids = nullptr, *sorted_dkeys = nullptr;       // [nv][N], set by bin_a
 };
 static size_t bin_a_bytes(int nv, int N) {
     const size_t nn = (size_t)nv * N;
@@ -270,6 +270,7 @@ static int bin_a(BinA& b, unsigned long long* host_totals, cudaStream_t s) {
                                 b.minkey_stride, false, s)) return 1; }
     STAGE_CHECK(b.dbg, s, "depth sort");
     b.sorted_ids = in_alt ? b.ids_alt : b.ids;
+    b.sorted_dkeys = in_alt ? b.dkeys_alt : b.dkeys;
     { StageTimer t(2, s);
     if (gs_scan_gather_seg_u32(b.tiles, b.sorted_ids, b.offsets, b.totals, b.N, b.nv, b.scan_scratch, s)) return 1; }
     GS_CUDA_CHECK(cudaMemcpyAsync(host_totals, b.totals, (size_t)b.nv * 8, cudaMemcpyDeviceToHost, s));
@@ -279,7 +280,10 @@ static int bin_a(BinA& b, unsigned long long* host_totals, cudaStream_t s) {
 static int view_spans(int nv, const unsigned long long* host_totals, ViewSpans& vs) {
     vs.n = nv; vs.base[0] = 0;
     for (int v = 0; v < nv; v++) {
-        if (host_totals[v] >= (1ull << 30)) { gs_set_error("too many (tile,splat) pairs in one view: %llu", host_totals[v]); return 1; }
+        if (host_totals[v] > (unsigned long long)GS_MAX_SEG_KEYS) {
+            gs_set_error("too many (tile,splat) pairs in one view: %llu (at most %lld)", host_totals[v], (long long)GS_MAX_SEG_KEYS);
+            return 1;
+        }
         vs.base[v + 1] = vs.base[v] + (int64_t)host_totals[v];
     }
     return 0;
@@ -634,6 +638,51 @@ PackedPtrs carve_packed(float* base, size_t N, size_t M, bool with_m2d) {
     return p;
 }
 
+// Workspace of one view chunk of the multi-view step: [VB][N] preprocess outputs and depth sort, binning scratch and
+// [VB][tiles][2] ranges, in five grow-only regions.
+struct ChunkWS { SplatRec* recs; SplatGrad* sg; int32_t* radii; uint32_t *minkeys, *ranges; uint4* spans; BinA bin; };
+int chunk_ws_setup(ChunkWS& w, Region& r_recs, Region& r_sg, Region& r_u32, Region& r_spans, Region& r_bin, int VB, int N,
+                   int ntiles, bool tight, cudaStream_t s) {
+    const size_t nvb = (size_t)VB * N;
+    if (Slot::ensure(r_recs, nvb * sizeof(SplatRec), s) || Slot::ensure(r_sg, nvb * sizeof(SplatGrad), s) ||
+        Slot::ensure(r_u32, nvb * 4 * 4 + 256 * 4, s) ||
+        Slot::ensure(r_bin, bin_a_bytes(VB, N) + Carver::need((size_t)VB * ntiles * 2, 4), s)) return 1;
+    if (tight && Slot::ensure(r_spans, nvb * sizeof(uint4), s)) return 1;
+    uint32_t* u32 = (uint32_t*)r_u32.p;
+    w.recs = (SplatRec*)r_recs.p; w.sg = (SplatGrad*)r_sg.p; w.radii = (int32_t*)u32;
+    w.minkeys = u32 + 4 * nvb;        // [VB] stride 2 words
+    w.spans = tight ? (uint4*)r_spans.p : nullptr;
+    w.bin.tiles = u32 + nvb; w.bin.dkeys = u32 + 2 * nvb; w.bin.ids = u32 + 3 * nvb;
+    w.bin.minkeys = w.minkeys; w.bin.minkey_stride = 2;
+    Carver cb(r_bin.p);
+    w.ranges = cb.take<uint32_t>((size_t)VB * ntiles * 2);
+    carve_bin_a(cb, w.bin, VB, N);
+    return 0;
+}
+// First half of a chunk's projection and binning (views_chunk: its nv views): preprocess, depth sort, scan, and the
+// D2H of the views' pair counts to host_totals.  geom_only: colours follow from gs_launch_sh_colour_multi.
+int chunk_bin_a(ChunkWS& w, const float* views_chunk, int nv, int W, int H, int sh_degree, float scale_modifier, int N,
+                int M, const PackedPtrs& par, int geom_only, unsigned long long* host_totals, cudaStream_t s) {
+    GS_CUDA_CHECK(cudaMemsetAsync(w.minkeys, 0xFF, 256 * 4, s));
+    { StageTimer t(0, s);
+    if (gs_launch_preprocess_multi(views_chunk, nv, W, H, sh_degree, scale_modifier, N, M, par.means, par.shs, par.colors,
+                                   par.opac, par.scales, par.rots, w.recs, w.radii, w.bin.tiles, w.bin.dkeys, w.bin.ids,
+                                   w.minkeys, w.spans, s, geom_only)) return 1; }
+    w.bin.nv = nv;
+    return bin_a(w.bin, host_totals, s);
+}
+size_t chunk_pairs_bytes(int nv, int64_t P) { return Carver::need(P, 4) * 2 + bin_b_scratch_bytes(nv, P); }
+// Second half, once the host has the chunk's pair bases vs (view_spans): the pair lists o carved from `pairs`
+// (chunk_pairs_bytes), ranges, emit, tile sort.
+int chunk_bin_b(ChunkWS& w, const ViewSpans& vs, void* pairs, BinB& o, int tiles_x, int tiles_y, cudaStream_t s) {
+    const int64_t P = vs.base[vs.n];
+    Carver cp(pairs);
+    o.point_list = cp.take<uint32_t>(P); o.tile_keys = cp.take<uint32_t>(P);
+    carve_bin_b_scratch(cp, o, vs.n, P);
+    GS_CUDA_CHECK(cudaMemsetAsync(w.ranges, 0, (size_t)vs.n * tiles_x * tiles_y * 2 * 4, s));
+    return bin_b(w.bin, vs, tiles_x, tiles_y, w.recs, w.spans, o, w.ranges, s);
+}
+
 // Device-resident core.  views_host gives tanfov per view (host side), views_dev the matrices.
 // Views are handled in chunks of <= VB.  Per chunk, on the aux stream: ONE multi-view preprocess pass over the
 // Gaussians (parameters read once), then the batched binning of all its views (segmented depth sort, gather-scan,
@@ -682,29 +731,14 @@ int step_core(int V, int H, int W, int sh_degree, float scale_modifier, const fl
     // order (bwd(k-1) before pre(k+1)) protects their reuse.
     const StepChunks chunks(V);
     const int nchunks = chunks.nchunks, VB = chunks.VB;
-    const size_t nvb = (size_t)VB * N;
     const bool tight = g_tile_culling.load() >= 1;
     const bool late = O.shs_ready && par.shs && !par.colors;
     if (O.shs_ready && !late) GS_CUDA_CHECK(cudaStreamWaitEvent(user, O.shs_ready, 0));
-    struct WS { SplatRec* recs; SplatGrad* sg; int32_t* radii; uint32_t *minkeys, *ranges; uint4* spans; BinA bin; } ws[2];
+    ChunkWS ws[2];
     const int nsets = nchunks > 1 ? 2 : 1;
-    const size_t ranges_bytes = Carver::need((size_t)VB * ntiles * 2, 4);
-    for (int i = 0; i < nsets; i++) {
-        if (Slot::ensure(C.ws_recs[i], nvb * sizeof(SplatRec), user) || Slot::ensure(C.ws_sg[i], nvb * sizeof(SplatGrad), user) ||
-            Slot::ensure(C.ws_u32[i], nvb * 4 * 4 + 256 * 4, user) ||
-            Slot::ensure(C.ws_bin[i], bin_a_bytes(VB, N) + ranges_bytes, user)) return 1;
-        if (tight && Slot::ensure(C.ws_spans[i], nvb * sizeof(uint4), user)) return 1;
-        uint32_t* u32 = (uint32_t*)C.ws_u32[i].p;
-        WS& w = ws[i];
-        w.recs = (SplatRec*)C.ws_recs[i].p; w.sg = (SplatGrad*)C.ws_sg[i].p; w.radii = (int32_t*)u32;
-        w.minkeys = u32 + 4 * nvb;        // [VB] stride 2 words
-        w.spans = tight ? (uint4*)C.ws_spans[i].p : nullptr;
-        w.bin.tiles = u32 + nvb; w.bin.dkeys = u32 + 2 * nvb; w.bin.ids = u32 + 3 * nvb;
-        w.bin.minkeys = w.minkeys; w.bin.minkey_stride = 2;
-        Carver cb(C.ws_bin[i].p);
-        w.ranges = cb.take<uint32_t>((size_t)VB * ntiles * 2);
-        carve_bin_a(cb, w.bin, VB, N);
-    }
+    for (int i = 0; i < nsets; i++)
+        if (chunk_ws_setup(ws[i], C.ws_recs[i], C.ws_sg[i], C.ws_u32[i], C.ws_spans[i], C.ws_bin[i], VB, N, ntiles, tight,
+                           user)) return 1;
     cudaStream_t aux = C.aux_stream;
     // everything is ordered after the caller's stream
     GS_CUDA_CHECK(cudaEventRecord(C.evFork, user));
@@ -716,14 +750,8 @@ int step_core(int V, int H, int W, int sh_degree, float scale_modifier, const fl
     // first half of chunk k's projection and binning on the aux stream: preprocess, depth sort, scan, pair counts D2H
     auto enqueue_pre = [&](int k) -> int {
         const int v0 = k * VB, nv = std::min(VB, V - v0);
-        WS& w = ws[k & (nsets - 1)];
-        GS_CUDA_CHECK(cudaMemsetAsync(w.minkeys, 0xFF, 256 * 4, aux));
-        { StageTimer t(0, aux);
-        if (gs_launch_preprocess_multi(views_dev + (size_t)v0 * 40, nv, W, H, sh_degree, scale_modifier, N, M, par.means,
-                                       par.shs, par.colors, par.opac, par.scales, par.rots, w.recs, w.radii, w.bin.tiles,
-                                       w.bin.dkeys, w.bin.ids, w.minkeys, w.spans, aux, late ? 1 : 0)) return 1; }
-        w.bin.nv = nv;
-        if (bin_a(w.bin, C.host_totals[k & 1], aux)) return 1;
+        if (chunk_bin_a(ws[k & (nsets - 1)], views_dev + (size_t)v0 * 40, nv, W, H, sh_degree, scale_modifier, N, M, par,
+                        late ? 1 : 0, C.host_totals[k & 1], aux)) return 1;
         GS_CUDA_CHECK(cudaEventRecord(C.evBinA[k & 1], aux));
         return 0;
     };
@@ -731,20 +759,15 @@ int step_core(int V, int H, int W, int sh_degree, float scale_modifier, const fl
     auto enqueue_bin = [&](int k) -> int {
         const int v0 = k * VB, nv = std::min(VB, V - v0);
         const int q = k & (nsets - 1);
-        WS& w = ws[q];
+        ChunkWS& w = ws[q];
         GS_CUDA_CHECK(cudaEventSynchronize(C.evBinA[k & 1]));
         ViewSpans& vs = vsp[k & 1];
         if (view_spans(nv, C.host_totals[k & 1], vs)) return 1;
         const int64_t P = vs.base[nv];
         rendered += P;
         // grow-only: the pair lists of all the chunk's views live until its last composite backward
-        if (Slot::ensure(C.ws_pairs[q], Carver::need(P, 4) * 2 + bin_b_scratch_bytes(nv, P), aux)) return 1;
-        Carver cp(C.ws_pairs[q].p);
-        BinB& o = pairs[k & 1];
-        o.point_list = cp.take<uint32_t>(P); o.tile_keys = cp.take<uint32_t>(P);
-        carve_bin_b_scratch(cp, o, nv, P);
-        GS_CUDA_CHECK(cudaMemsetAsync(w.ranges, 0, (size_t)nv * ntiles * 2 * 4, aux));
-        if (bin_b(w.bin, vs, tiles_x, tiles_y, w.recs, w.spans, o, w.ranges, aux)) return 1;
+        if (Slot::ensure(C.ws_pairs[q], chunk_pairs_bytes(nv, P), aux)) return 1;
+        if (chunk_bin_b(w, vs, C.ws_pairs[q].p, pairs[k & 1], tiles_x, tiles_y, aux)) return 1;
         if (late) {
             GS_CUDA_CHECK(cudaStreamWaitEvent(aux, O.shs_ready, 0));
             if (gs_launch_sh_colour_multi(views_dev + (size_t)v0 * 40, nv, sh_degree, N, M, par.means, par.shs, w.radii, w.recs, aux)) return 1;
@@ -757,7 +780,7 @@ int step_core(int V, int H, int W, int sh_degree, float scale_modifier, const fl
     if (!rc) rc = enqueue_bin(0);
     for (int k = 0; k < nchunks && !rc; k++) {
         const int v0 = k * VB, nv = std::min(VB, V - v0);
-        const WS& w = ws[k & (nsets - 1)];
+        const ChunkWS& w = ws[k & (nsets - 1)];
         const ViewSpans& vs = vsp[k & 1];
         const BinB& o = pairs[k & 1];
         // the slot streams continue after this chunk's binning ...
@@ -1015,6 +1038,84 @@ int32_t gs_b200_render_views(int32_t V, int32_t H, int32_t W, int32_t sh_degree,
     StepOpts o; o.forward_only = true; o.radii_out = radii;
     return step_core(V, H, W, sh_degree, scale_modifier, views_host, views_dev, N, M, par, nullptr, nullptr, grd, images,
                      num_rendered_out, s, nullptr, &o);
+}
+
+// ---- test entries of the binning stage ----------------------------------------------------------------------
+
+int32_t gs_b200_debug_sort_segmented(uint32_t* keys, uint32_t* keys_alt, uint32_t* vals, uint32_t* vals_alt,
+                                     const int64_t* seg_off, int32_t nseg, int32_t begin_bit, int32_t end_bit,
+                                     const uint32_t* key_bias, int32_t bias_stride, int32_t* result_in_alt, void* stream_) {
+    cudaStream_t s = (cudaStream_t)stream_;
+    if (!seg_off || nseg < 1 || nseg > GS_MAX_SEGS || !result_in_alt) { gs_set_error("debug_sort_segmented: bad argument"); return 1; }
+    SortSegs sg; sg.n = nseg;
+    for (int i = 0; i <= nseg; i++) sg.off[i] = seg_off[i];
+    void* scratch = nullptr;
+    const size_t bytes = gs_sort_seg_scratch_bytes(nseg, std::max<int64_t>(seg_off[nseg], 0));
+    GS_CUDA_CHECK(cudaMallocAsync(&scratch, bytes, s));
+    int r = 0;
+    const int rc = gs_sort_pairs_segmented(keys, keys_alt, vals, vals_alt, sg, begin_bit, end_bit, scratch, &r, key_bias,
+                                           bias_stride, false, s);
+    cudaFreeAsync(scratch, s);
+    *result_in_alt = r;
+    return rc;
+}
+
+// The multi-view step's projection and binning, as step_core runs them (StepChunks, chunk_ws_setup, chunk_bin_a,
+// view_spans, chunk_bin_b), on `stream` alone, with every intermediate list copied out.
+int32_t gs_b200_debug_bin_views(int32_t V, int32_t H, int32_t W, int32_t sh_degree, float scale_modifier,
+                                const float* views_dev, int32_t N, int32_t M, const float* means3D, const float* shs,
+                                const float* opacities, const float* scales, const float* rotations, int32_t tight,
+                                int32_t* radii, uint32_t* tiles_touched, uint32_t* spans, uint32_t* sorted_dkeys,
+                                uint32_t* sorted_ids, uint32_t* offsets, int64_t* totals, uint32_t* ranges,
+                                uint32_t* point_list, uint32_t* tile_keys, void* stream_) {
+    cudaStream_t s = (cudaStream_t)stream_;
+    if (V <= 0 || N <= 0 || M < (sh_degree + 1) * (sh_degree + 1) || M > 16 || !views_dev || !means3D || !shs ||
+        !opacities || !scales || !rotations || !radii || !tiles_touched || (tight && !spans) || !sorted_dkeys ||
+        !sorted_ids || !offsets || !totals || (point_list && (!tile_keys || !ranges))) {
+        gs_set_error("debug_bin_views: bad argument"); return 1;
+    }
+    struct Regions {
+        Region r[6];
+        ~Regions() { for (Region& x : r) if (x.p) cudaFree(x.p); }
+    } R;
+    const int tiles_x = (W + GS_TILE - 1) / GS_TILE, tiles_y = (H + GS_TILE - 1) / GS_TILE, ntiles = tiles_x * tiles_y;
+    const StepChunks ch(V);
+    ChunkWS w;
+    if (chunk_ws_setup(w, R.r[0], R.r[1], R.r[2], R.r[3], R.r[4], ch.VB, N, ntiles, tight != 0, s)) return 1;
+    PackedPtrs par; par.means = (float*)means3D; par.shs = (float*)shs; par.opac = (float*)opacities;
+    par.scales = (float*)scales; par.rots = (float*)rotations; par.m2d = nullptr;
+    unsigned long long host_totals[GS_MAX_SEGS];
+    int64_t pair0 = 0;        // the chunk's first pair in point_list / tile_keys
+    for (int k = 0; k < ch.nchunks; k++) {
+        const int v0 = k * ch.VB, nv = std::min(ch.VB, V - v0);
+        const size_t o = (size_t)v0 * N, n = (size_t)nv * N;
+        if (chunk_bin_a(w, views_dev + (size_t)v0 * 40, nv, W, H, sh_degree, scale_modifier, N, M, par, 0, host_totals, s)) return 1;
+        GS_CUDA_CHECK(cudaMemcpyAsync(radii + o, w.radii, n * 4, cudaMemcpyDeviceToDevice, s));
+        GS_CUDA_CHECK(cudaMemcpyAsync(tiles_touched + o, w.bin.tiles, n * 4, cudaMemcpyDeviceToDevice, s));
+        if (tight) GS_CUDA_CHECK(cudaMemcpyAsync(spans + 4 * o, w.spans, n * 16, cudaMemcpyDeviceToDevice, s));
+        GS_CUDA_CHECK(cudaMemcpyAsync(sorted_dkeys + o, w.bin.sorted_dkeys, n * 4, cudaMemcpyDeviceToDevice, s));
+        GS_CUDA_CHECK(cudaMemcpyAsync(sorted_ids + o, w.bin.sorted_ids, n * 4, cudaMemcpyDeviceToDevice, s));
+        GS_CUDA_CHECK(cudaMemcpyAsync(offsets + o, w.bin.offsets, n * 4, cudaMemcpyDeviceToDevice, s));
+        GS_CUDA_CHECK(cudaStreamSynchronize(s));
+        for (int j = 0; j < nv; j++) totals[v0 + j] = (int64_t)host_totals[j];
+        ViewSpans vs;
+        if (view_spans(nv, host_totals, vs)) return 1;
+        if (!point_list) continue;      // first call of two: the caller sizes the pair lists from `totals`
+        const int64_t P = vs.base[nv];
+        if (Slot::ensure(R.r[5], chunk_pairs_bytes(nv, P), s)) return 1;
+        // a pair slot the emit leaves unwritten keeps this value through the sort
+        GS_CUDA_CHECK(cudaMemsetAsync(R.r[5].p, 0xFF, chunk_pairs_bytes(nv, P), s));
+        BinB b;
+        if (chunk_bin_b(w, vs, R.r[5].p, b, tiles_x, tiles_y, s)) return 1;
+        GS_CUDA_CHECK(cudaMemcpyAsync(ranges + (size_t)v0 * ntiles * 2, w.ranges, (size_t)nv * ntiles * 8, cudaMemcpyDeviceToDevice, s));
+        if (P > 0) {
+            GS_CUDA_CHECK(cudaMemcpyAsync(point_list + pair0, b.point_list, (size_t)P * 4, cudaMemcpyDeviceToDevice, s));
+            GS_CUDA_CHECK(cudaMemcpyAsync(tile_keys + pair0, b.tile_keys, (size_t)P * 4, cudaMemcpyDeviceToDevice, s));
+        }
+        pair0 += P;
+        GS_CUDA_CHECK(cudaStreamSynchronize(s));
+    }
+    return 0;
 }
 
 int32_t gs_b200_step_host(int32_t V, int32_t H, int32_t W, int32_t sh_degree, float scale_modifier,

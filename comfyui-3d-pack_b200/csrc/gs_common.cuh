@@ -224,6 +224,9 @@ int gs_launch_densify_stats(int, const float*, const int32_t*, float*, float*, f
 // launch per digit pass.  The multi-view step sorts the depth keys and the tile keys of all views of a chunk so.
 constexpr int GS_MAX_SEGS = 16;
 struct SortSegs { int n; int64_t off[GS_MAX_SEGS + 1]; };
+// Most keys one segment may hold: the sort's look-back status words keep a digit's running count in their low 30 bits.
+// The binning refuses a view with more (tile, splat) pairs before it allocates them (view_spans in gs_capi.cu).
+constexpr int64_t GS_MAX_SEG_KEYS = (1ll << 30) - 1;
 
 size_t gs_sort_scratch_bytes(int64_t n);
 size_t gs_sort_seg_scratch_bytes(int nseg, int64_t total_n);

@@ -153,9 +153,13 @@ __device__ __forceinline__ void project_view(const ViewK& vk, int deg, int M, fl
     const float disc = sqrtf(fmaxf(mid * mid - det, 0.1f));
     const float lam1 = mid + disc, lam2 = mid - disc;
     const float radf = ceilf(3.0f * sqrtf(fmaxf(lam1, lam2)));
+    // A NaN extent (a NaN or non-positive-definite covariance: an overflowed scale, a bad cov3D_precomp) is culled.
+    // Converted, it would be radius 0 with a one-tile rect that the emit (radius > 0 only) never fills.  Finite
+    // extents are >= 1 here; +inf, like any extent past INT_MAX, saturates to INT_MAX: a full-screen square.
+    if (!(radf > 0.0f)) return;
     const float px = ((ndcx + 1.0f) * (float)vk.W - 1.0f) * 0.5f;
     const float py = ((ndcy + 1.0f) * (float)vk.H - 1.0f) * 0.5f;
-    const int rad_i = (int)radf;
+    const int rad_i = __float2int_rz(radf);
     int x0, y0, x1, y1;
     get_rect(px, py, rad_i, vk.tiles_x, vk.tiles_y, x0, y0, x1, y1);
     const int area = (x1 - x0) * (y1 - y0);

@@ -25,6 +25,7 @@ constexpr int RS_PART = RS_THREADS * RS_ITEMS;   // 4096 pairs per partition
 constexpr int RS_RADIX = 256;
 constexpr int RS_MAX_PASSES = 4;
 constexpr uint32_t FLAG_AGG = 1u << 30, FLAG_PFX = 2u << 30, VAL_MASK = (1u << 30) - 1;
+static_assert(GS_MAX_SEG_KEYS <= (int64_t)VAL_MASK, "a segment's digit counts must fit the status word");
 
 // ---- segments -----------------------------------------------------------------
 // The keys are sorted as nseg independent segments [off[i], off[i+1]) of one array (the multi-view step sorts
@@ -437,7 +438,7 @@ int gs_sort_pairs_segmented(uint32_t* keys, uint32_t* keys_alt, uint32_t* vals, 
         if (i == segs.n) break;
         const int64_t len = segs.off[i + 1] - segs.off[i];
         if (len < 0) { gs_set_error("sort: segment %d has negative length", i); return 1; }
-        if (len >= (int64_t)VAL_MASK) { gs_set_error("sort: n too large"); return 1; }
+        if (len > GS_MAX_SEG_KEYS) { gs_set_error("sort: segment %d has %lld keys (at most %lld)", i, (long long)len, (long long)GS_MAX_SEG_KEYS); return 1; }
         maxlen = std::max(maxlen, len);
         parts += (len + RS_PART - 1) / RS_PART;
     }

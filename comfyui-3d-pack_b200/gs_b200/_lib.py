@@ -55,6 +55,12 @@ lib.gs_b200_debug_preprocess_backward.argtypes = [C.POINTER(View), C.c_int32, C.
 lib.gs_b200_debug_preprocess_backward_multi.restype = C.c_int32
 lib.gs_b200_debug_preprocess_backward_multi.argtypes = [C.c_int32] * 4 + [C.c_float, _P, C.c_int32, C.c_int32] + \
     [_P] * 7 + [C.c_int32, _P]
+lib.gs_b200_debug_sort_segmented.restype = C.c_int32
+lib.gs_b200_debug_sort_segmented.argtypes = [_P] * 4 + [_P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int32,
+                                                         C.POINTER(C.c_int32), _P]
+lib.gs_b200_debug_bin_views.restype = C.c_int32
+lib.gs_b200_debug_bin_views.argtypes = [C.c_int32] * 4 + [C.c_float, _P, C.c_int32, C.c_int32] + [_P] * 5 + \
+    [C.c_int32] + [_P] * 10 + [_P]
 lib.gs_b200_step_view_chunks.restype = C.c_int32
 lib.gs_b200_step_view_chunks.argtypes = [C.c_int32, _P]
 lib.gs_b200_sort_scratch_bytes.restype = C.c_size_t
@@ -256,7 +262,8 @@ lib.gs_b200_composite_bwd_occupancy.argtypes = [C.POINTER(C.c_int32), C.POINTER(
 EXPORTS = ["gs_b200_set_grad_sink", "gs_b200_composite_bwd_occupancy", "gs_b200_image_loss", "gs_b200_step_device_train", "gs_b200_step_device_hook", "gs_b200_render_views", "gs_b200_set_tile_culling", "gs_b200_get_tile_culling", "gs_b200_step_device", "gs_b200_step_host_dev_grads", "gs_b200_launch_count", "gs_b200_profile_enable", "gs_b200_profile_read",
            "gs_b200_abi_version", "gs_b200_last_error", "gs_b200_rasterize_forward", "gs_b200_rasterize_backward",
            "gs_b200_state_free", "gs_b200_debug_sorted_keys", "gs_b200_debug_preprocess_backward",
-           "gs_b200_debug_preprocess_backward_multi", "gs_b200_step_view_chunks", "gs_b200_sort_scratch_bytes",
+           "gs_b200_debug_preprocess_backward_multi", "gs_b200_step_view_chunks", "gs_b200_debug_sort_segmented",
+           "gs_b200_debug_bin_views", "gs_b200_sort_scratch_bytes",
            "gs_b200_sort_pairs_u32", "gs_b200_knn_mean_dist2", "gs_b200_step_host"] + SCATTER_EXPORTS + CR_EXPORTS + \
     UVBAKE_EXPORTS
 

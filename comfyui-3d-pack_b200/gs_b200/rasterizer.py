@@ -17,6 +17,7 @@ the sm_90a library behind include/gs_b200.h.  No CPU path exists.
 from typing import NamedTuple, Optional
 import ctypes as C
 
+import numpy as np
 import torch
 import torch.nn as nn
 
@@ -269,6 +270,62 @@ def sort_pairs_u32(keys: torch.Tensor, vals: Optional[torch.Tensor], begin_bit: 
         _lib.check(_lib.lib.gs_b200_sort_pairs_u32(_ptr(k0), _ptr(k1), _ptr(v0), _ptr(v1), n, begin_bit, end_bit,
                                                    _ptr(scratch), C.byref(alt), _stream()))
     return (k1, v1) if alt.value else (k0, v0)
+
+
+def sort_pairs_segmented(keys: torch.Tensor, vals: torch.Tensor, seg_off, begin_bit: int = 0, end_bit: int = 32,
+                         key_bias: Optional[torch.Tensor] = None, bias_stride: int = 0):
+    """The binning's segmented sort (tests): segments [seg_off[i], seg_off[i+1]) of int32-viewed u32 keys + values,
+    each sorted on its own by (key - key_bias[i * bias_stride]) mod 2^32; returns sorted (keys, vals)."""
+    assert keys.is_cuda and keys.dtype == torch.int32 and keys.is_contiguous() and vals.shape == keys.shape
+    k0, v0 = keys.clone(), vals.clone()
+    k1, v1 = torch.empty_like(k0), torch.empty_like(v0)
+    off = (C.c_int64 * len(seg_off))(*[int(x) for x in seg_off])
+    alt = C.c_int32(0)
+    with torch.cuda.device(keys.device):
+        _lib.check(_lib.lib.gs_b200_debug_sort_segmented(_ptr(k0), _ptr(k1), _ptr(v0), _ptr(v1), off, len(seg_off) - 1,
+                                                         begin_bit, end_bit, _ptr(key_bias), bias_stride, C.byref(alt),
+                                                         _stream()))
+    return (k1, v1) if alt.value else (k0, v0)
+
+
+def bin_views(views: torch.Tensor, H: int, W: int, sh_degree: int, scale_modifier: float, means3D, shs, opacities,
+              scales, rotations, tight: bool, lists: bool = True) -> dict:
+    """The multi-view step's projection and binning (tests): views [V, 40] as the step entries take them.  Returns
+    per view [V, N] radii, tiles_touched, spans [V, N, 4] (tight only), sorted_dkeys, sorted_ids, offsets and
+    totals [V] (int64, host); with `lists` also ranges [V, tiles, 2] and point_list / tile_keys, each a list of V
+    tensors.  u32 values are returned as int64."""
+    V, N, M = views.shape[0], means3D.shape[0], shs.shape[1]
+    dev = means3D.device
+    ntiles = ((W + 15) // 16) * ((H + 15) // 16)
+    ins = [_dev_f32(t, "input") for t in (views, means3D, shs, opacities, scales, rotations)]
+    i32 = lambda *sh: torch.empty(*sh, dtype=torch.int32, device=dev)        # noqa: E731
+    out = dict(radii=i32(V, N), tiles_touched=i32(V, N), spans=i32(V, N, 4) if tight else None, sorted_dkeys=i32(V, N),
+               sorted_ids=i32(V, N), offsets=i32(V, N))
+    totals = (C.c_int64 * V)()
+
+    def call(pl, tk, rg):
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib.gs_b200_debug_bin_views(
+                V, H, W, sh_degree, scale_modifier, _ptr(ins[0]), N, M, *(_ptr(t) for t in ins[1:]), int(bool(tight)),
+                *(_ptr(out[k]) for k in ("radii", "tiles_touched", "spans", "sorted_dkeys", "sorted_ids", "offsets")),
+                totals, _ptr(rg), _ptr(pl), _ptr(tk), _stream()))
+        torch.cuda.synchronize(dev)
+    call(None, None, None)
+    tot = [int(t) for t in totals]
+    res = {}
+    if lists:
+        P = sum(tot)
+        pl, tk, rg = i32(max(P, 1)), i32(max(P, 1)), i32(V, ntiles, 2)
+        call(pl, tk, rg)
+        if [int(t) for t in totals] != tot:
+            raise RuntimeError("bin_views: pair totals changed between the two calls")
+        cut = np.cumsum([0] + tot)
+        res["point_list"] = [pl[cut[v]:cut[v + 1]].long() & 0xFFFFFFFF for v in range(V)]
+        res["tile_keys"] = [tk[cut[v]:cut[v + 1]].long() & 0xFFFFFFFF for v in range(V)]
+        res["ranges"] = rg.long() & 0xFFFFFFFF
+    res.update({k: None if v is None else v.long() & 0xFFFFFFFF for k, v in out.items()})
+    res["radii"], res["totals"] = out["radii"], tot
+    return res
 
 
 def knn_mean_dist2(points: torch.Tensor) -> torch.Tensor:

@@ -154,6 +154,26 @@ int32_t gs_b200_debug_preprocess_backward_multi(
     int32_t V, int32_t H, int32_t W, int32_t sh_degree, float scale_modifier, const float* views_dev,
     int32_t N, int32_t M, const float* means3D, const float* shs, const float* scales, const float* rotations,
     const int32_t* radii, const double* splat_grads, float* grads_dev, int32_t nparts, void* stream);
+/* Tests of the binning stage.
+ * debug_sort_segmented: the segmented onesweep sort of the binning, nseg (1..16) segments [seg_off[i], seg_off[i+1])
+ * of ping-pong key/value arrays (seg_off on the host), on bits [begin_bit, end_bit); key_bias (device, may be NULL):
+ * segment i's keys are sorted as key - key_bias[i * bias_stride] (mod 2^32).  *result_in_alt = 1 when the result is
+ * in keys_alt / vals_alt.
+ * debug_bin_views: the projection and binning of the gs_b200_step_* entries, through the same code: views_dev [V][40]
+ * and the parameters as theirs, the views in the step's chunks, tile culling on (tight = 1) or off.  Outputs, [V][N]:
+ * radii, tiles_touched, spans (uint32 x 4 per Gaussian, tight only), the depth-sorted keys and Gaussian ids, the
+ * exclusive scan offsets; totals[V] (host) the pairs of each view.  Call it first with point_list = NULL to learn the
+ * totals; a second call with point_list / tile_keys [sum of totals] (view after view) and ranges [V][tiles][2] also
+ * returns the lists.  The pair buffers are filled with 0xFFFFFFFF before the emit, so an unwritten slot shows. */
+int32_t gs_b200_debug_sort_segmented(uint32_t* keys, uint32_t* keys_alt, uint32_t* vals, uint32_t* vals_alt,
+                                     const int64_t* seg_off, int32_t nseg, int32_t begin_bit, int32_t end_bit,
+                                     const uint32_t* key_bias, int32_t bias_stride, int32_t* result_in_alt, void* stream);
+int32_t gs_b200_debug_bin_views(int32_t V, int32_t H, int32_t W, int32_t sh_degree, float scale_modifier,
+                                const float* views_dev, int32_t N, int32_t M, const float* means3D, const float* shs,
+                                const float* opacities, const float* scales, const float* rotations, int32_t tight,
+                                int32_t* radii, uint32_t* tiles_touched, uint32_t* spans, uint32_t* sorted_dkeys,
+                                uint32_t* sorted_ids, uint32_t* offsets, int64_t* totals, uint32_t* ranges,
+                                uint32_t* point_list, uint32_t* tile_keys, void* stream);
 /* The view chunks of the multi-view step for V views: bounds[k] is the first view of chunk k, bounds[nchunks] = V
  * (bounds holds at least V + 1 entries).  Returns nchunks, or -1 on a bad argument.  Host only. */
 int32_t gs_b200_step_view_chunks(int32_t V, int32_t* bounds);
