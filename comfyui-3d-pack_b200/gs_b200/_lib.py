@@ -245,6 +245,27 @@ lib.gs_b200_scatter_backward.argtypes = [_I, _I, _P, _I, _L, _P, _P, _P, _P, _P,
 SCATTER_EXPORTS = ["gs_b200_scatter_index_range", "gs_b200_scatter_scratch_bytes", "gs_b200_scatter_forward",
                    "gs_b200_scatter_backward"]
 
+PN2_FPS_ONCHIP_MAX = 16384
+lib.gs_b200_pn2_furthest_point_sample.restype = _I
+lib.gs_b200_pn2_furthest_point_sample.argtypes = [_I, _I, _I, _P, _P, _P, _P]
+lib.gs_b200_pn2_ball_query.restype = _I
+lib.gs_b200_pn2_ball_query.argtypes = [_I, _I, _I, _I, _F, _P, _P, _P, _P]
+lib.gs_b200_pn2_three_nn.restype = _I
+lib.gs_b200_pn2_three_nn.argtypes = [_I, _I, _I, _P, _P, _P, _P, _P]
+lib.gs_b200_pn2_gather.restype = _I
+lib.gs_b200_pn2_gather.argtypes = [_I, _I, _I, _I, _P, _P, _P, _P]
+lib.gs_b200_pn2_three_interpolate.restype = _I
+lib.gs_b200_pn2_three_interpolate.argtypes = [_I, _I, _I, _I, _P, _P, _P, _P, _P]
+lib.gs_b200_pn2_backward_scratch_bytes.restype = C.c_size_t
+lib.gs_b200_pn2_backward_scratch_bytes.argtypes = [_I, _I, _I, _L, _I]
+lib.gs_b200_pn2_gather_backward.restype = _I
+lib.gs_b200_pn2_gather_backward.argtypes = [_I, _I, _I, _L, _P, _P, _P, _P, _P]
+lib.gs_b200_pn2_three_interpolate_backward.restype = _I
+lib.gs_b200_pn2_three_interpolate_backward.argtypes = [_I, _I, _I, _I, _P, _P, _P, _P, _P, _P]
+PN2_EXPORTS = ["gs_b200_pn2_furthest_point_sample", "gs_b200_pn2_ball_query", "gs_b200_pn2_three_nn",
+               "gs_b200_pn2_gather", "gs_b200_pn2_three_interpolate", "gs_b200_pn2_backward_scratch_bytes",
+               "gs_b200_pn2_gather_backward", "gs_b200_pn2_three_interpolate_backward"]
+
 NSTAGES = 9
 STAGE_NAMES = ["preprocess", "depth_sort", "scan", "emit", "tile_sort", "ranges", "composite_fwd",
                "composite_bwd", "preprocess_bwd"]
@@ -265,7 +286,7 @@ EXPORTS = ["gs_b200_set_grad_sink", "gs_b200_composite_bwd_occupancy", "gs_b200_
            "gs_b200_debug_preprocess_backward_multi", "gs_b200_step_view_chunks", "gs_b200_debug_sort_segmented",
            "gs_b200_debug_bin_views", "gs_b200_sort_scratch_bytes",
            "gs_b200_sort_pairs_u32", "gs_b200_knn_mean_dist2", "gs_b200_step_host"] + SCATTER_EXPORTS + CR_EXPORTS + \
-    UVBAKE_EXPORTS
+    UVBAKE_EXPORTS + PN2_EXPORTS
 
 
 def last_error() -> str:

@@ -228,6 +228,47 @@ int32_t gs_b200_scatter_backward(int32_t op, int32_t ndim, const int64_t* shape_
                                  const int64_t* grad_out_strides_host, const int64_t* argmax, const void* fwd_scratch,
                                  float* grad_src, float* grad_out_mean, void* stream);
 
+/* ---- pointnet2_ops replacement (furthest_point_sample, gather / grouping_operation, ball_query, three_nn,
+ * three_interpolate) --------------------------------------------------------------------------------------------------
+ * Every pointer is a contiguous device array: coordinates fp32 [.., 3], features fp32 [B, C, ..], indices int32.
+ * Squared distances are ((dx*dx + dy*dy) + dz*dz) in fp32, one rounding per operation (no FMA contraction).
+ *   furthest_point_sample  xyz [B,N,3] -> idx_out [B,npoint].  idx_out[.,0] = 0; running distances start at 1e10;
+ *       step s sets temp[k] = fminf(temp[k], d2(k, last)) and picks the largest temp, the smallest index on ties.
+ *       A point with (x*x + y*y) + z*z <= 1e-3 (fp32, compared as double) is never updated nor picked; when no point
+ *       can be picked the pick is 0, so npoint > N is defined.  N > GS_B200_PN2_FPS_ONCHIP_MAX needs `temp`, B*N
+ *       floats of scratch (otherwise it may be NULL).
+ *   ball_query  xyz [B,N,3], new_xyz [B,npoint,3] -> idx_out [B,npoint,nsample]: the first nsample k, ascending, with
+ *       d2 < radius*radius (fp32); slots past the last hit repeat the first hit, and a query without a hit is all 0.
+ *   three_nn  unknown [B,n,3], known [B,m,3] -> dist [B,n,3], idx [B,n,3]: the three smallest (d2, k) in lexicographic
+ *       order among k with d2 < +inf (NaN never enters), dist = sqrtf(d2) correctly rounded; unfilled slots (+inf, 0).
+ *   gather  features [B,C,N], idx [B,M] -> out [B,C,M]: out[b,c,j] = features[b,c,idx[b,j]], 0 where idx lies outside
+ *       [0,N).  gather_operation (M = npoint) and grouping_operation (M = npoint*nsample) share it.
+ *   three_interpolate  features [B,C,m], idx [B,n,3], weight [B,n,3] -> out [B,C,n] =
+ *       (w0*f0 + w1*f1) + w2*f2, with f = 0 for an idx outside [0,m).
+ * Backward (fp32): grad_features [B, C, N + 1], where slot N collects the entries whose idx lies outside [0,N) and is
+ * discarded by the caller.  Each slot is +0 plus its contributions in ascending position (j for gather, 3i + k for
+ * three_interpolate, whose contribution is grad_out[b,c,i] * weight[b,i,k] rounded once) through
+ * gs_b200_scatter_forward's fold: no fp32 atomics, no host read, the same bits on every run.  scratch:
+ * gs_b200_pn2_backward_scratch_bytes(B, C, N, M, three) bytes (M = the gather's M, or n with three = 1;
+ * 0 = invalid arguments).  Fewer than 2^31 elements per tensor and 2^30 index entries (B*M, B*n*3). */
+#define GS_B200_PN2_FPS_ONCHIP_MAX 16384
+int32_t gs_b200_pn2_furthest_point_sample(int32_t B, int32_t N, int32_t npoint, const float* xyz, int32_t* idx_out,
+                                          float* temp, void* stream);
+int32_t gs_b200_pn2_ball_query(int32_t B, int32_t N, int32_t npoint, int32_t nsample, float radius, const float* xyz,
+                               const float* new_xyz, int32_t* idx_out, void* stream);
+int32_t gs_b200_pn2_three_nn(int32_t B, int32_t n, int32_t m, const float* unknown, const float* known, float* dist,
+                             int32_t* idx, void* stream);
+int32_t gs_b200_pn2_gather(int32_t B, int32_t C, int32_t N, int32_t M, const float* features, const int32_t* idx,
+                           float* out, void* stream);
+int32_t gs_b200_pn2_three_interpolate(int32_t B, int32_t C, int32_t m, int32_t n, const float* features,
+                                      const int32_t* idx, const float* weight, float* out, void* stream);
+size_t gs_b200_pn2_backward_scratch_bytes(int32_t B, int32_t C, int32_t N, int64_t M, int32_t three);
+int32_t gs_b200_pn2_gather_backward(int32_t B, int32_t C, int32_t N, int64_t M, const float* grad_out,
+                                    const int32_t* idx, float* grad_features, void* scratch, void* stream);
+int32_t gs_b200_pn2_three_interpolate_backward(int32_t B, int32_t C, int32_t m, int32_t n, const float* grad_out,
+                                               const int32_t* idx, const float* weight, float* grad_features,
+                                               void* scratch, void* stream);
+
 /* Multi-view optimisation step with DEVICE-resident buffers: V x (forward + backward), gradients
  * summed over views into `grads` (zeroed first), packed as
  *   means3D[N,3] | shs[N,M,3] | opacities[N] | scales[N,3] | rotations[N,4] | means2D[N,3]

@@ -83,3 +83,32 @@ for tool in memcheck racecheck; do
   timeout 1200 compute-sanitizer --tool $tool --error-exitcode 9 --launch-timeout 0 python /tmp/ub_case.py 2>&1 | tail -6
   echo "ub $tool rc=$?"
 done
+
+# pointnet2_ops (pn2_ops.cu): FPS on-chip and global-memory kernels, ball query, three-NN, gather / grouping and
+# three-interpolate forward and backward, with out-of-range indices; memcheck and racecheck
+cat > /tmp/pn2_case.py <<'PY'
+import sys, os
+ROOT = os.getcwd(); sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "comfyui-3d-pack_b200"))
+import torch
+from pointnet2_ops import pointnet2_utils as U
+dev = torch.device("cuda:0")
+g = torch.Generator(device=dev).manual_seed(0)
+for N in (1000, 5000, 16384, 17000):
+    xyz = torch.rand(2, N, 3, generator=g, device=dev) * 2 - 1
+    idx = U.furthest_point_sample(xyz, 64)
+print("fps", int(idx.sum()))
+xyz = torch.rand(1, 3000, 3, generator=g, device=dev)
+print("ball", int(U.ball_query(0.2, 32, xyz, xyz[:, :100].contiguous()).sum()))
+d, i = U.three_nn(xyz, xyz[:, :50].contiguous())
+f = torch.randn(1, 8, 3000, device=dev, requires_grad=True)
+bad = torch.randint(-5, 3005, (1, 200, 16), generator=g, device=dev, dtype=torch.int32)
+U.grouping_operation(f, bad).sum().backward()
+U.gather_operation(f, bad[:, :, 0].contiguous()).sum().backward()
+fi = torch.randn(1, 8, 50, device=dev, requires_grad=True)
+U.three_interpolate(fi, i, torch.rand(1, 3000, 3, device=dev)).sum().backward()
+torch.cuda.synchronize(); print("pn2 ok", float(f.grad.abs().sum()), float(fi.grad.abs().sum()))
+PY
+for tool in memcheck racecheck; do
+  timeout 1200 compute-sanitizer --tool $tool --error-exitcode 9 --launch-timeout 0 python /tmp/pn2_case.py 2>&1 | tail -6
+  echo "pn2 $tool rc=$?"
+done
