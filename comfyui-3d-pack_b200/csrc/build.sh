@@ -13,7 +13,7 @@ $NVCC $COMMON -fmad=false -c dr_raster.cu -o build/dr_raster.o & pids+=($!)
 $NVCC $COMMON -fmad=false -c cr_raster.cu -o build/cr_raster.o & pids+=($!)
 $NVCC $COMMON -fmad=false -c uv_bake.cu -o build/uv_bake.o & pids+=($!)
 $NVCC $COMMON -fmad=false -c pn2_ops.cu -o build/pn2_ops.o & pids+=($!)
-for f in gs_sort gs_binning gs_composite gs_backward gs_knn gs_train gs_densify gs_loss gs_capi dr_ops dr_capi ngp_ops ngp_mlp ngp_capi ngp_mcubes ngp_flexicubes ngp_dmc gs_scatter; do
+for f in gs_sort gs_binning gs_composite gs_backward gs_knn gs_train gs_densify gs_loss gs_capi dr_ops dr_capi ngp_ops ngp_mlp ngp_capi ngp_mcubes ngp_flexicubes ngp_dmc gs_scatter sp_conv; do
   $NVCC $COMMON -c $f.cu -o build/$f.o & pids+=($!)
 done
 for p in "${pids[@]}"; do wait $p; done

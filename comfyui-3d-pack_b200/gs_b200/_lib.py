@@ -266,6 +266,23 @@ PN2_EXPORTS = ["gs_b200_pn2_furthest_point_sample", "gs_b200_pn2_ball_query", "g
                "gs_b200_pn2_gather", "gs_b200_pn2_three_interpolate", "gs_b200_pn2_backward_scratch_bytes",
                "gs_b200_pn2_gather_backward", "gs_b200_pn2_three_interpolate_backward"]
 
+SPCONV_F32, SPCONV_F16 = 0, 1
+SPCONV_MAX_ROWS = (1 << 30) - 1
+lib.gs_b200_spconv_map_scratch_bytes.restype = C.c_size_t
+lib.gs_b200_spconv_map_scratch_bytes.argtypes = [_L]
+lib.gs_b200_spconv_build_map.restype = _I
+lib.gs_b200_spconv_build_map.argtypes = [_L, _I, _I, _I, _I] + [_P] * 7
+lib.gs_b200_spconv_forward.restype = _I
+lib.gs_b200_spconv_forward.argtypes = [_I, _L, _I, _I, _I] + [_P] * 7
+lib.gs_b200_spconv_backward_scratch_bytes.restype = C.c_size_t
+lib.gs_b200_spconv_backward_scratch_bytes.argtypes = [_I, _L, _I, _I, _I]
+lib.gs_b200_spconv_dgrad.restype = _I
+lib.gs_b200_spconv_dgrad.argtypes = [_I, _L, _I, _I, _I] + [_P] * 9
+lib.gs_b200_spconv_wgrad.restype = _I
+lib.gs_b200_spconv_wgrad.argtypes = [_I, _L, _I, _I, _I] + [_P] * 7
+SPCONV_EXPORTS = ["gs_b200_spconv_map_scratch_bytes", "gs_b200_spconv_build_map", "gs_b200_spconv_forward",
+                  "gs_b200_spconv_backward_scratch_bytes", "gs_b200_spconv_dgrad", "gs_b200_spconv_wgrad"]
+
 NSTAGES = 9
 STAGE_NAMES = ["preprocess", "depth_sort", "scan", "emit", "tile_sort", "ranges", "composite_fwd",
                "composite_bwd", "preprocess_bwd"]
@@ -286,7 +303,7 @@ EXPORTS = ["gs_b200_set_grad_sink", "gs_b200_composite_bwd_occupancy", "gs_b200_
            "gs_b200_debug_preprocess_backward_multi", "gs_b200_step_view_chunks", "gs_b200_debug_sort_segmented",
            "gs_b200_debug_bin_views", "gs_b200_sort_scratch_bytes",
            "gs_b200_sort_pairs_u32", "gs_b200_knn_mean_dist2", "gs_b200_step_host"] + SCATTER_EXPORTS + CR_EXPORTS + \
-    UVBAKE_EXPORTS + PN2_EXPORTS
+    UVBAKE_EXPORTS + PN2_EXPORTS + SPCONV_EXPORTS
 
 
 def last_error() -> str:

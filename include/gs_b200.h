@@ -269,6 +269,52 @@ int32_t gs_b200_pn2_three_interpolate_backward(int32_t B, int32_t C, int32_t m, 
                                                const int32_t* idx, const float* weight, float* grad_features,
                                                void* scratch, void* stream);
 
+/* ---- spconv replacement (spconv.pytorch.SubMConv3d, kernel size 1 or 3, stride 1, dilation 1) ------------------------
+ * Rows: indices int32 [N, 4] = (b, x, y, z) in any order (16-byte aligned), features [N, Cin], out [N, Cout] in the same
+ * row order; spatial shape [X, Y, Z], batch size B.  weight [Cout, k, k, k, Cin] (spconv 2.x's KRSC layout), bias [Cout]
+ * or NULL.  With r = (k - 1) / 2 and offset o = (o0, o1, o2) in {-r..r}^3 (linear index ((o0+r)*k + o1+r)*k + o2+r):
+ *   out[i, :] = bias + sum over o of W[:, o + r, :] . in[j, :]
+ * where j is the row at (b, x+o0, y+o1, z+o2); a neighbour that is absent, outside [0,X)x[0,Y)x[0,Z) or in another batch
+ * item contributes nothing (cross-correlation: on a fully occupied grid this is F.conv3d(dense, W.permute(0,4,1,2,3),
+ * padding=r) with the spatial axes in index-column order).  Duplicate coordinates: every lookup resolves to the smallest
+ * row among them.  A row with b outside [0,B) or a coordinate outside the grid is nobody's neighbour and has none.
+ * k = 1 is a per-row GEMM without a map: every row reads its own features.
+ * Neighbour map (k = 3), built on the device with no host read:
+ *   nbr int32 [N, 27]: the neighbour's row, -1 when absent.  mask uint32 [N]: bit o set when nbr[i, o] >= 0; bit 31 set
+ *   when row i repeats the coordinate of a smaller row.  sorted_keys / sorted_rows uint32 [N]: the rows' keys
+ *   ((b*X + x)*Y + y)*Z + z (0xffffffff for an invalid row) in stable ascending order and their rows (bit 31 marks an
+ *   invalid row); dgrad reads them.  B*X*Y*Z must not exceed 2^32.  scratch: gs_b200_spconv_map_scratch_bytes(N).
+ * dtype GS_B200_SPCONV_F16: fp16 features / weight / bias / out, fp16 x fp16 products summed in fp32 on tensor cores,
+ *   bias added in fp32, one rounding to fp16.  GS_B200_SPCONV_F32: fp32 FFMA (not TF32), one fmaf chain per output
+ *   over (offset ascending, input channel ascending), then + bias.
+ * Backward (same dtype as the forward):
+ *   dgrad  grad_features [N, Cin] = the forward loop run with W^T and mirrored offsets over the same map (the map of an
+ *          odd-k submanifold conv is symmetric); each coordinate's gradient reaching its smallest row is first summed
+ *          over the coordinate's duplicate rows (fp32, ascending row, one rounding), and the duplicates get 0.
+ *   wgrad  grad_weight [Cout, k, k, k, Cin] = sum over rows i of grad_out[i] (x) in[nbr[i, o]], and grad_bias [Cout] =
+ *          sum of grad_out rows (either may be NULL): fp32 partials over fixed row chunks chosen from the shape alone,
+ *          added in ascending chunk order, one rounding to the dtype.
+ *   scratch: gs_b200_spconv_backward_scratch_bytes(...) bytes, for either call (0 = invalid arguments).
+ * No fp32 atomics anywhere: every output and gradient has the same bits on every run.  N <= GS_B200_SPCONV_MAX_ROWS,
+ * fewer than 2^31 elements in features, out and weight. */
+enum { GS_B200_SPCONV_F32 = 0, GS_B200_SPCONV_F16 = 1 };
+#define GS_B200_SPCONV_MAX_ROWS 1073741823
+size_t gs_b200_spconv_map_scratch_bytes(int64_t N);
+int32_t gs_b200_spconv_build_map(int64_t N, int32_t B, int32_t X, int32_t Y, int32_t Z, const int32_t* indices,
+                                 int32_t* nbr, uint32_t* mask, uint32_t* sorted_keys, uint32_t* sorted_rows,
+                                 void* scratch, void* stream);
+int32_t gs_b200_spconv_forward(int32_t dtype, int64_t N, int32_t Cin, int32_t Cout, int32_t k, const void* features,
+                               const int32_t* nbr, const uint32_t* mask, const void* weight, const void* bias,
+                               void* out, void* stream);
+size_t gs_b200_spconv_backward_scratch_bytes(int32_t dtype, int64_t N, int32_t Cin, int32_t Cout, int32_t k);
+int32_t gs_b200_spconv_dgrad(int32_t dtype, int64_t N, int32_t Cin, int32_t Cout, int32_t k, const void* grad_out,
+                             const int32_t* nbr, const uint32_t* mask, const uint32_t* sorted_keys,
+                             const uint32_t* sorted_rows, const void* weight, void* grad_features, void* scratch,
+                             void* stream);
+int32_t gs_b200_spconv_wgrad(int32_t dtype, int64_t N, int32_t Cin, int32_t Cout, int32_t k, const void* features,
+                             const void* grad_out, const int32_t* nbr, void* grad_weight, void* grad_bias,
+                             void* scratch, void* stream);
+
 /* Multi-view optimisation step with DEVICE-resident buffers: V x (forward + backward), gradients
  * summed over views into `grads` (zeroed first), packed as
  *   means3D[N,3] | shs[N,M,3] | opacities[N] | scales[N,3] | rotations[N,4] | means2D[N,3]

@@ -112,3 +112,30 @@ for tool in memcheck racecheck; do
   timeout 1200 compute-sanitizer --tool $tool --error-exitcode 9 --launch-timeout 0 python /tmp/pn2_case.py 2>&1 | tail -6
   echo "pn2 $tool rc=$?"
 done
+
+# spconv (sp_conv.cu): neighbour map with duplicates and rows outside the grid, fp16 (vector and element-wise loads)
+# and fp32 forward, dgrad with the duplicate fold, wgrad / dbias over several chunks; memcheck and racecheck
+cat > /tmp/sp_case.py <<'PY'
+import sys, os
+ROOT = os.getcwd(); sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "comfyui-3d-pack_b200"))
+import torch
+from gs_b200 import spconv as S
+from oracle import spconv_oracle as O
+dev = torch.device("cuda:0")
+for name, ind, spatial, B in O.edge_sets():
+    m = S.build_map(torch.from_numpy(ind).to(dev), spatial, B, 3)
+    for dt, cin in ((torch.float16, 40), (torch.float16, 13), (torch.float32, 13)):
+        x = torch.randn(len(ind), cin, device=dev, dtype=dt, requires_grad=True)
+        w = torch.randn(24, 3, 3, 3, cin, device=dev, dtype=dt, requires_grad=True)
+        b = torch.randn(24, device=dev, dtype=dt, requires_grad=True)
+        S.submconv3d(x, w, b, m).float().sum().backward()
+ind = torch.from_numpy(O.subdivide(O.sphere_shell(24))).to(dev)
+x = torch.randn(len(ind), 16, device=dev, requires_grad=True)
+w = torch.randn(16, 3, 3, 3, 16, device=dev, requires_grad=True)
+S.submconv3d(x, w, None, S.build_map(ind, (48, 48, 48), 1, 3)).sum().backward()
+torch.cuda.synchronize(); print("sp ok", float(w.grad.abs().sum()))
+PY
+for tool in memcheck racecheck; do
+  timeout 1200 compute-sanitizer --tool $tool --error-exitcode 9 --launch-timeout 0 python /tmp/sp_case.py 2>&1 | tail -6
+  echo "sp $tool rc=$?"
+done
