@@ -17,22 +17,14 @@ this module.
   misread there); all work goes on the current stream (the reference runs its resolve pass on the legacy default
   stream); CPU tensors raise RuntimeError and other dtypes TypeError (no CPU path).
 """
-import ctypes as C
 
 import torch
 
 from . import _lib
+from ._lib import ptr, stream
 from . import scatter as _scatter
 
 OCCLUSION_TRUNCATION = 1e-6
-
-
-def _P(t):
-    return C.c_void_p(t.data_ptr() if t is not None and t.numel() else None)
-
-
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _cuda(t, what, dtypes):
@@ -75,9 +67,9 @@ def rasterize_image(V, F, D, width, height, occlusion_truncation, use_depth_prio
         findices = torch.empty(H, W, dtype=torch.int32, device=dev)
         bary = torch.empty(H, W, 3, dtype=torch.float32, device=dev)
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        _lib.check(_lib.lib.dr_b200_cr_rasterize(_P(v), v.shape[0], _P(f), f.shape[0], _P(d), H, W,
-                                                 float(occlusion_truncation), _P(findices), _P(bary), _P(scratch),
-                                                 _stream()))
+        _lib.check(_lib.lib.dr_b200_cr_rasterize(ptr(v), v.shape[0], ptr(f), f.shape[0], ptr(d), H, W,
+                                                 float(occlusion_truncation), ptr(findices), ptr(bary), ptr(scratch),
+                                                 stream()))
     return [findices, bary]
 
 
@@ -96,10 +88,10 @@ class _InterpolateFn(torch.autograd.Function):
         c0 = c0.contiguous()
         npix = findices.numel()
         out = torch.empty(*findices.shape, Cn, dtype=torch.float32, device=col.device)
-        args = (_P(c0), NV, Cn, _P(findices), int(findices.dtype == torch.float32), _P(barycentric), _P(tri),
+        args = (ptr(c0), NV, Cn, ptr(findices), int(findices.dtype == torch.float32), ptr(barycentric), ptr(tri),
                 int(tri.dtype == torch.int64), tri.shape[0], npix)
         with torch.cuda.device(col.device):
-            _lib.check(_lib.lib.dr_b200_cr_interpolate_fwd(*args, _P(out), _stream()))
+            _lib.check(_lib.lib.dr_b200_cr_interpolate_fwd(*args, ptr(out), stream()))
         ctx.save_for_backward(c0, barycentric, findices, tri)
         ctx.col_shape = tuple(col.shape)
         return out.view(1, *out.shape)
@@ -118,8 +110,8 @@ class _InterpolateFn(torch.autograd.Function):
         gcol = None
         with torch.cuda.device(dev):
             _lib.check(_lib.lib.dr_b200_cr_interpolate_bwd(
-                _P(c0), NV, Cn, _P(findices), int(findices.dtype == torch.float32), _P(barycentric), _P(tri),
-                int(tri.dtype == torch.int64), tri.shape[0], npix, _P(g), _P(gb), _P(contrib), _P(cidx), _stream()))
+                ptr(c0), NV, Cn, ptr(findices), int(findices.dtype == torch.float32), ptr(barycentric), ptr(tri),
+                int(tri.dtype == torch.int64), tri.shape[0], npix, ptr(g), ptr(gb), ptr(contrib), ptr(cidx), stream()))
             if want_col:
                 gcol = torch.zeros(ctx.col_shape, dtype=torch.float32, device=dev)
                 if npix:

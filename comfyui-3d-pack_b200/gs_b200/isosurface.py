@@ -32,7 +32,7 @@ def marching_cubes(volume, iso):
     vol = volume.to(torch.float32).contiguous()
     X, Y, Z = vol.shape
     with torch.cuda.device(dev):
-        stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+        stream = _lib.stream()
         scratch = torch.empty(int(_lib.lib.ngp_b200_mcubes_scratch_bytes(X, Y, Z)), dtype=torch.uint8, device=dev)
         totals = torch.empty(3, dtype=torch.int64, device=dev)
         _lib.check(_lib.lib.ngp_b200_mcubes_count(_P(vol), X, Y, Z, float(iso), _P(totals), _P(scratch), stream))
@@ -109,7 +109,7 @@ class _FlexiCubesFn(torch.autograd.Function):
         attrs, sc, nc = _attr_arg(attrs, x.shape[0])
         opt = lambda t: _P(t) if t is not None else None
         with torch.cuda.device(dev):
-            stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+            stream = _lib.stream()
             scratch = torch.empty(int(_lib.lib.ngp_b200_flexicubes_scratch_bytes(*R)), dtype=torch.uint8, device=dev)
             totals = torch.empty(4, dtype=torch.int64, device=dev)
             _lib.check(_lib.lib.ngp_b200_flexicubes_count(_P(s), *R, _P(totals), _P(scratch), stream))
@@ -151,7 +151,7 @@ class _FlexiCubesFn(torch.autograd.Function):
         gat = new(attrs is not None and need[5], (x.shape[0], nc))
         opt = lambda t: _P(t) if t is not None else None
         with torch.cuda.device(dev):
-            stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+            stream = _lib.stream()
             args = (_P(x), _P(s), opt(beta), sb, opt(alpha), sa, opt(gamma), sg, *R, float(ws), int(training), host,
                     _P(verts), _P(gverts), _P(gldev), opt(gx), opt(gs), opt(gb), opt(ga), opt(gg))
             if attrs is None:
@@ -281,7 +281,7 @@ class _DiffDMCFn(torch.autograd.Function):
         X, Y, Z = grid.shape
         opt = lambda t: _P(t) if t is not None else None
         with torch.cuda.device(dev):
-            stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+            stream = _lib.stream()
             scratch = torch.empty(int(_lib.lib.ngp_b200_dmc_scratch_bytes(X, Y, Z)), dtype=torch.uint8, device=dev)
             totals = torch.empty(3, dtype=torch.int64, device=dev)
             _lib.check(_lib.lib.ngp_b200_dmc_count(_P(grid), X, Y, Z, iso, _P(totals), _P(scratch), stream))
@@ -312,7 +312,7 @@ class _DiffDMCFn(torch.autograd.Function):
         gd = torch.empty_like(deform) if deform is not None and need[1] else None
         opt = lambda t: _P(t) if t is not None else None
         with torch.cuda.device(dev):
-            stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+            stream = _lib.stream()
             work = torch.empty(max(int(_lib.lib.ngp_b200_dmc_backward_workspace_bytes(X, Y, Z)), 1), dtype=torch.uint8,
                                device=dev)
             _lib.check(_lib.lib.ngp_b200_dmc_backward(_P(grid), opt(deform), X, Y, Z, iso, int(normalize),

@@ -12,12 +12,9 @@ import weakref
 import torch
 
 from . import _lib
+from ._lib import stream
 
 _P = lambda t: None if t is None else C.c_void_p(t.data_ptr())
-
-
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _f32(t, what):
@@ -65,7 +62,7 @@ class _Rasterize(torch.autograd.Function):
         with torch.cuda.device(dev):
             rast = torch.empty(B, H, W, 4, device=dev); db = torch.empty(B, H, W, 4, device=dev)
             scratch = torch.empty(int(_lib.lib.dr_b200_rasterize_scratch_bytes(B, F, H, W)), dtype=torch.uint8, device=dev)
-            _lib.check(_lib.lib.dr_b200_rasterize_fwd(_P(p), _P(t), B, V, F, H, W, _P(rast), _P(db), _P(scratch), _stream()))
+            _lib.check(_lib.lib.dr_b200_rasterize_fwd(_P(p), _P(t), B, V, F, H, W, _P(rast), _P(db), _P(scratch), stream()))
         ctx.save_for_backward(p, t, rast)
         ctx.dims = (B, V, F, H, W)
         ctx.mark_non_differentiable(db)
@@ -79,7 +76,7 @@ class _Rasterize(torch.autograd.Function):
         if g_rast is not None and F > 0:
             g = _f32(g_rast, "grad")
             with torch.cuda.device(p.device):
-                _lib.check(_lib.lib.dr_b200_rasterize_bwd(_P(p), _P(t), B, V, F, H, W, _P(rast), _P(g), _P(d_pos), _stream()))
+                _lib.check(_lib.lib.dr_b200_rasterize_bwd(_P(p), _P(t), B, V, F, H, W, _P(rast), _P(g), _P(d_pos), stream()))
         return d_pos, None, None, None
 
 
@@ -106,7 +103,7 @@ class _Interpolate(torch.autograd.Function):
         with torch.cuda.device(dev):
             out = torch.empty(B, H, W, A, device=dev)
             out_da = torch.empty(B, H, W, 2 * A, device=dev) if want_da else None
-            _lib.check(_lib.lib.dr_b200_interpolate_fwd(_P(a), aB, _P(r), _P(t), _P(db), B, V, F, H, W, A, _P(out), _P(out_da), _stream()))
+            _lib.check(_lib.lib.dr_b200_interpolate_fwd(_P(a), aB, _P(r), _P(t), _P(db), B, V, F, H, W, A, _P(out), _P(out_da), stream()))
         ctx.save_for_backward(a, r, t, db)
         ctx.dims = (aB, B, V, F, H, W, A, want_da)
         if want_da:
@@ -125,7 +122,7 @@ class _Interpolate(torch.autograd.Function):
         d_db = torch.empty_like(r) if gda is not None else None
         with torch.cuda.device(dev):
             _lib.check(_lib.lib.dr_b200_interpolate_bwd(_P(a), aB, _P(r), _P(t), _P(db if gda is not None else None), B, V, F, H, W, A,
-                                                        _P(g), _P(gda), _P(d_attr), _P(d_rast), _P(d_db), _stream()))
+                                                        _P(g), _P(gda), _P(d_attr), _P(d_rast), _P(d_db), stream()))
         return d_attr, d_rast, None, d_db, None
 
 
@@ -152,7 +149,7 @@ class _Texture(torch.autograd.Function):
         dev = u.device
         with torch.cuda.device(dev):
             out = torch.empty(B, H, W, Cc, device=dev)
-            _lib.check(_lib.lib.dr_b200_texture_fwd(_P(t), tB, Ht, Wt, Cc, _P(u), B, H, W, boundary, _P(out), _stream()))
+            _lib.check(_lib.lib.dr_b200_texture_fwd(_P(t), tB, Ht, Wt, Cc, _P(u), B, H, W, boundary, _P(out), stream()))
         ctx.save_for_backward(t, u)
         ctx.boundary = boundary
         return out
@@ -165,7 +162,7 @@ class _Texture(torch.autograd.Function):
         g = _f32(g_out, "grad")
         d_tex = torch.zeros_like(t); d_uv = torch.empty_like(u)
         with torch.cuda.device(u.device):
-            _lib.check(_lib.lib.dr_b200_texture_bwd(_P(t), tB, Ht, Wt, Cc, _P(u), B, H, W, ctx.boundary, _P(g), _P(d_tex), _P(d_uv), _stream()))
+            _lib.check(_lib.lib.dr_b200_texture_bwd(_P(t), tB, Ht, Wt, Cc, _P(u), B, H, W, ctx.boundary, _P(g), _P(d_tex), _P(d_uv), stream()))
         return d_tex, d_uv, None
 
 
@@ -248,7 +245,7 @@ def get_topology(tri, n_vertices):
     if F > 0:
         with torch.cuda.device(t.device):
             scratch = torch.empty(int(_lib.lib.dr_b200_topology_scratch_bytes(F)), dtype=torch.uint8, device=t.device)
-            _lib.check(_lib.lib.dr_b200_edge_opposites(_P(t), F, int(n_vertices), _P(opp), _P(scratch), _stream()))
+            _lib.check(_lib.lib.dr_b200_edge_opposites(_P(t), F, int(n_vertices), _P(opp), _P(scratch), stream()))
     tid = id(tri)
     try:
         _TOPO_CACHE[tid] = (weakref.ref(tri, lambda _r, tid=tid: _TOPO_CACHE.pop(tid, None)), key, opp)
@@ -265,7 +262,7 @@ class _Antialias(torch.autograd.Function):
         V = p.shape[1]; F = t.shape[0]
         with torch.cuda.device(c.device):
             out = torch.empty_like(c)
-            _lib.check(_lib.lib.dr_b200_antialias_fwd(_P(c), _P(r), _P(p), _P(t), _P(opp), B, V, F, H, W, Cc, _P(out), _stream()))
+            _lib.check(_lib.lib.dr_b200_antialias_fwd(_P(c), _P(r), _P(p), _P(t), _P(opp), B, V, F, H, W, Cc, _P(out), stream()))
         ctx.save_for_backward(c, r, p, t, opp)
         return out
 
@@ -277,7 +274,7 @@ class _Antialias(torch.autograd.Function):
         g = _f32(g_out, "grad")
         d_color = torch.empty_like(c); d_pos = torch.zeros_like(p)
         with torch.cuda.device(c.device):
-            _lib.check(_lib.lib.dr_b200_antialias_bwd(_P(c), _P(r), _P(p), _P(t), _P(opp), B, V, F, H, W, Cc, _P(g), _P(d_color), _P(d_pos), _stream()))
+            _lib.check(_lib.lib.dr_b200_antialias_bwd(_P(c), _P(r), _P(p), _P(t), _P(opp), B, V, F, H, W, Cc, _P(g), _P(d_color), _P(d_pos), stream()))
         return d_color, None, d_pos, None, None
 
 

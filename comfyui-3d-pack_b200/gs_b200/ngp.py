@@ -10,6 +10,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
+from ._lib import stream
 
 _P = lambda t: None if t is None else C.c_void_p(t.data_ptr())
 
@@ -31,10 +32,6 @@ def _rand(shape, device):
     return torch.rand(shape, generator=_RNG, dtype=torch.float32).to(device)
 
 
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
 def _f32c(t):
     if not t.is_cuda:
         raise RuntimeError("CUDA tensor required (gs_b200 NGP ops have no CPU path)")
@@ -53,7 +50,7 @@ class _GridEncode(torch.autograd.Function):
         out = torch.empty(N, enc.num_levels * enc.level_dim, device=xs.device)
         with torch.cuda.device(xs.device):
             _lib.check(_lib.lib.ngp_b200_grid_encode_fwd(_P(xs), N, _P(e), enc._off_ptr, enc.num_levels, float(enc._bound_call),
-                                                         float(enc.per_level_scale), int(enc.base_resolution), _P(out), _stream()))
+                                                         float(enc.per_level_scale), int(enc.base_resolution), _P(out), stream()))
         ctx.save_for_backward(xs)
         ctx.enc = enc
         ctx.bound = float(enc._bound_call)
@@ -68,7 +65,7 @@ class _GridEncode(torch.autograd.Function):
         d_emb = torch.zeros(ctx.shape, device=xs.device)
         with torch.cuda.device(xs.device):
             _lib.check(_lib.lib.ngp_b200_grid_encode_bwd(_P(xs), xs.shape[0], enc._off_ptr, enc.num_levels, ctx.bound,
-                                                         float(enc.per_level_scale), int(enc.base_resolution), _P(g), _P(d_emb), _stream()))
+                                                         float(enc.per_level_scale), int(enc.base_resolution), _P(g), _P(d_emb), stream()))
         return None, d_emb, None
 
 
@@ -124,7 +121,7 @@ class GridEncoder(nn.Module):
         with torch.cuda.device(dev):
             _lib.check(_lib.lib.ngp_b200_grid_tv_grad(_P(x), x.shape[0], _P(_f32c(self.embeddings)), self._off_ptr, self.num_levels,
                                                       float(bound), float(self.per_level_scale), int(self.base_resolution),
-                                                      float(weight), _P(self.embeddings.grad), _stream()))
+                                                      float(weight), _P(self.embeddings.grad), stream()))
 
 
 # ------------------------------------------------------------------------------------------------ kiui.nn / kiui.op / kiui.cam
@@ -138,7 +135,7 @@ class _FusedMLP2(torch.autograd.Function):
         H, Dout = w1.shape[0], w2.shape[0]
         y = torch.empty(N, Dout, device=xs.device)
         with torch.cuda.device(xs.device):
-            _lib.check(_lib.lib.ngp_b200_mlp2_fwd(_P(xs), N, Din, H, Dout, _P(w1), _P(w2), _P(y), _stream()))
+            _lib.check(_lib.lib.ngp_b200_mlp2_fwd(_P(xs), N, Din, H, Dout, _P(w1), _P(w2), _P(y), stream()))
         ctx.save_for_backward(xs, w1, w2)
         ctx.need_gx = x.requires_grad
         return y
@@ -152,7 +149,7 @@ class _FusedMLP2(torch.autograd.Function):
         gx = torch.empty_like(xs) if ctx.need_gx else None
         gw1 = torch.zeros_like(w1); gw2 = torch.zeros_like(w2)
         with torch.cuda.device(xs.device):
-            _lib.check(_lib.lib.ngp_b200_mlp2_bwd(_P(xs), N, Din, H, Dout, _P(w1), _P(w2), _P(g), _P(gx), _P(gw1), _P(gw2), _stream()))
+            _lib.check(_lib.lib.ngp_b200_mlp2_bwd(_P(xs), N, Din, H, Dout, _P(w1), _P(w2), _P(g), _P(gx), _P(gw1), _P(gw2), stream()))
         return gx, gw1, gw2
 
 
@@ -294,12 +291,12 @@ def march_rays(rays_o, rays_d, binary, aabb, near_plane, far_plane, dt, t_offset
         total = torch.zeros(1, dtype=torch.int64, device=dev)
         ap = C.c_void_p(aabb_np.ctypes.data)
         _lib.check(_lib.lib.ngp_b200_march_count(_P(ro), _P(rd), n, _P(b8), R, ap, float(near_plane), float(far_plane), float(dt),
-                                                 _P(toff), _P(counts), _P(offsets), _P(total), _P(scratch), _stream()))
+                                                 _P(toff), _P(counts), _P(offsets), _P(total), _P(scratch), stream()))
         S = int(total.item())
         ri = torch.empty(S, dtype=torch.int64, device=dev); ts = torch.empty(S, device=dev); te = torch.empty(S, device=dev)
         if S > 0:
             _lib.check(_lib.lib.ngp_b200_march_write(_P(ro), _P(rd), n, R, ap, float(near_plane), float(far_plane), float(dt),
-                                                     _P(toff), _P(offsets), _P(ri), _P(ts), _P(te), _P(scratch), _stream()))
+                                                     _P(toff), _P(offsets), _P(ri), _P(ts), _P(te), _P(scratch), stream()))
     return ri, ts, te
 
 
@@ -307,7 +304,7 @@ def _ranges(ray_indices, n_rays):
     ri = ray_indices.contiguous()
     rng = torch.empty(max(n_rays, 1), 2, dtype=torch.int32, device=ri.device)
     with torch.cuda.device(ri.device):
-        _lib.check(_lib.lib.ngp_b200_ray_ranges(_P(ri), ri.numel(), n_rays, _P(rng), _stream()))
+        _lib.check(_lib.lib.ngp_b200_ray_ranges(_P(ri), ri.numel(), n_rays, _P(rng), stream()))
     return rng
 
 
@@ -317,7 +314,7 @@ class _Weights(torch.autograd.Function):
         ts, te, sg = _f32c(t_starts), _f32c(t_ends), _f32c(sigmas)
         w = torch.empty_like(sg); tr = torch.empty_like(sg); al = torch.empty_like(sg)
         with torch.cuda.device(sg.device):
-            _lib.check(_lib.lib.ngp_b200_weights_fwd(_P(ts), _P(te), _P(sg), _P(ranges), n_rays, _P(w), _P(tr), _P(al), _stream()))
+            _lib.check(_lib.lib.ngp_b200_weights_fwd(_P(ts), _P(te), _P(sg), _P(ranges), n_rays, _P(w), _P(tr), _P(al), stream()))
         ctx.save_for_backward(ts, te, sg, ranges, tr, al)
         ctx.n_rays = n_rays
         return w, tr, al
@@ -329,7 +326,7 @@ class _Weights(torch.autograd.Function):
         f = lambda g: None if g is None else _f32c(g)
         with torch.cuda.device(sg.device):
             _lib.check(_lib.lib.ngp_b200_weights_bwd(_P(ts), _P(te), _P(sg), _P(ranges), ctx.n_rays, _P(tr), _P(al), _P(f(gw)), _P(f(gt)),
-                                                     _P(f(ga)), _P(d), _stream()))
+                                                     _P(f(ga)), _P(d), stream()))
         return None, None, d, None, None
 
 
@@ -352,7 +349,7 @@ class _Accumulate(torch.autograd.Function):
         Cc = 1 if v is None else v.shape[-1]
         out = torch.empty(n_rays, Cc, device=w.device)
         with torch.cuda.device(w.device):
-            _lib.check(_lib.lib.ngp_b200_accumulate_fwd(_P(w), _P(v), Cc, _P(ranges), n_rays, _P(out), _stream()))
+            _lib.check(_lib.lib.ngp_b200_accumulate_fwd(_P(w), _P(v), Cc, _P(ranges), n_rays, _P(out), stream()))
         ctx.save_for_backward(w, v, ray_indices)
         ctx.Cc = Cc
         return out
@@ -364,7 +361,7 @@ class _Accumulate(torch.autograd.Function):
         dw = torch.empty_like(w)
         dv = None if v is None else torch.empty_like(v)
         with torch.cuda.device(w.device):
-            _lib.check(_lib.lib.ngp_b200_accumulate_bwd(_P(w), _P(v), ctx.Cc, _P(ri.contiguous()), w.numel(), _P(g), _P(dw), _P(dv), _stream()))
+            _lib.check(_lib.lib.ngp_b200_accumulate_bwd(_P(w), _P(v), ctx.Cc, _P(ri.contiguous()), w.numel(), _P(g), _P(dw), _P(dv), stream()))
         return dw, dv, None, None, None
 
 

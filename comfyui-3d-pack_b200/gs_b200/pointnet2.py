@@ -13,19 +13,11 @@ states every rule), as the autograd Functions pointnet2_ops.pointnet2_utils defi
   0 in the forward and is skipped in the backward.
 - Work goes on the current stream of the inputs' device.  No CPU path.
 """
-import ctypes as C
 
 import torch
 
 from . import _lib
-
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr() if t is not None and t.numel() else None)
-
-
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+from ._lib import ptr, stream
 
 
 def _inputs(name, **named):
@@ -82,7 +74,7 @@ class FurthestPointSampling(torch.autograd.Function):
         with torch.cuda.device(xyz.device):
             out = torch.empty(B, npoint, dtype=torch.int32, device=xyz.device)
             temp = torch.empty(B * N, dtype=torch.float32, device=xyz.device) if N > _lib.PN2_FPS_ONCHIP_MAX else None
-            _lib.check(_lib.lib.gs_b200_pn2_furthest_point_sample(B, N, npoint, _ptr(xyz), _ptr(out), _ptr(temp), _stream()))
+            _lib.check(_lib.lib.gs_b200_pn2_furthest_point_sample(B, N, npoint, ptr(xyz), ptr(out), ptr(temp), stream()))
         ctx.mark_non_differentiable(out)
         return out
 
@@ -101,8 +93,8 @@ def _gather_backward(grad, idx, B, C_, N, M):
             raise RuntimeError(f"gs_b200: {_lib.last_error()}")
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         full = torch.empty(B, C_, N + 1, dtype=torch.float32, device=dev)
-        _lib.check(_lib.lib.gs_b200_pn2_gather_backward(B, C_, N, M, _ptr(grad), _ptr(idx), _ptr(full), _ptr(scratch),
-                                                        _stream()))
+        _lib.check(_lib.lib.gs_b200_pn2_gather_backward(B, C_, N, M, ptr(grad), ptr(idx), ptr(full), ptr(scratch),
+                                                        stream()))
     return full[:, :, :N]
 
 
@@ -120,7 +112,7 @@ class GatherOperation(torch.autograd.Function):
         M = idx.size(1)
         with torch.cuda.device(features.device):
             out = torch.empty(B, C_, M, dtype=torch.float32, device=features.device)
-            _lib.check(_lib.lib.gs_b200_pn2_gather(B, C_, N, M, _ptr(features), _ptr(idx), _ptr(out), _stream()))
+            _lib.check(_lib.lib.gs_b200_pn2_gather(B, C_, N, M, ptr(features), ptr(idx), ptr(out), stream()))
         ctx.save_for_backward(idx)
         ctx.dims = (B, C_, N, M)
         return out
@@ -145,7 +137,7 @@ class GroupingOperation(torch.autograd.Function):
         P, S = idx.shape[1:]
         with torch.cuda.device(features.device):
             out = torch.empty(B, C_, P, S, dtype=torch.float32, device=features.device)
-            _lib.check(_lib.lib.gs_b200_pn2_gather(B, C_, N, P * S, _ptr(features), _ptr(idx), _ptr(out), _stream()))
+            _lib.check(_lib.lib.gs_b200_pn2_gather(B, C_, N, P * S, ptr(features), ptr(idx), ptr(out), stream()))
         ctx.save_for_backward(idx)
         ctx.dims = (B, C_, N, P * S)
         return out
@@ -171,8 +163,8 @@ class BallQuery(torch.autograd.Function):
         P = new_xyz.size(1)
         with torch.cuda.device(xyz.device):
             out = torch.zeros(B, P, nsample, dtype=torch.int32, device=xyz.device)
-            _lib.check(_lib.lib.gs_b200_pn2_ball_query(B, N, P, nsample, float(radius), _ptr(xyz), _ptr(new_xyz),
-                                                       _ptr(out), _stream()))
+            _lib.check(_lib.lib.gs_b200_pn2_ball_query(B, N, P, nsample, float(radius), ptr(xyz), ptr(new_xyz),
+                                                       ptr(out), stream()))
         ctx.mark_non_differentiable(out)
         return out
 
@@ -196,7 +188,7 @@ class ThreeNN(torch.autograd.Function):
         with torch.cuda.device(unknown.device):
             dist = torch.empty(B, n, 3, dtype=torch.float32, device=unknown.device)
             idx = torch.empty(B, n, 3, dtype=torch.int32, device=unknown.device)
-            _lib.check(_lib.lib.gs_b200_pn2_three_nn(B, n, m, _ptr(unknown), _ptr(known), _ptr(dist), _ptr(idx), _stream()))
+            _lib.check(_lib.lib.gs_b200_pn2_three_nn(B, n, m, ptr(unknown), ptr(known), ptr(dist), ptr(idx), stream()))
         ctx.mark_non_differentiable(dist, idx)
         return dist, idx
 
@@ -222,8 +214,8 @@ class ThreeInterpolate(torch.autograd.Function):
         n = idx.size(1)
         with torch.cuda.device(features.device):
             out = torch.empty(B, C_, n, dtype=torch.float32, device=features.device)
-            _lib.check(_lib.lib.gs_b200_pn2_three_interpolate(B, C_, m, n, _ptr(features), _ptr(idx), _ptr(weight),
-                                                              _ptr(out), _stream()))
+            _lib.check(_lib.lib.gs_b200_pn2_three_interpolate(B, C_, m, n, ptr(features), ptr(idx), ptr(weight),
+                                                              ptr(out), stream()))
         ctx.save_for_backward(idx, weight)
         ctx.dims = (B, C_, m, n)
         return out
@@ -240,8 +232,8 @@ class ThreeInterpolate(torch.autograd.Function):
                 raise RuntimeError(f"gs_b200: {_lib.last_error()}")
             scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             full = torch.empty(B, C_, m + 1, dtype=torch.float32, device=dev)
-            _lib.check(_lib.lib.gs_b200_pn2_three_interpolate_backward(B, C_, m, n, _ptr(grad_out), _ptr(idx),
-                                                                       _ptr(weight), _ptr(full), _ptr(scratch), _stream()))
+            _lib.check(_lib.lib.gs_b200_pn2_three_interpolate_backward(B, C_, m, n, ptr(grad_out), ptr(idx),
+                                                                       ptr(weight), ptr(full), ptr(scratch), stream()))
         return full[:, :, :m], None, None
 
 

@@ -22,6 +22,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
+from ._lib import stream as _stream
 
 
 class GaussianRasterizationSettings(NamedTuple):
@@ -90,10 +91,6 @@ def _make_view(rs: GaussianRasterizationSettings, keep: list) -> _lib.View:
     return _lib.View(int(rs.image_height), int(rs.image_width), float(rs.tanfovx), float(rs.tanfovy),
                      bg.data_ptr(), float(rs.scale_modifier), vm.data_ptr(), pm.data_ptr(), int(rs.sh_degree),
                      cp.data_ptr(), int(bool(rs.prefiltered)), int(bool(rs.debug)))
-
-
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 class _RasterizeGaussians(torch.autograd.Function):

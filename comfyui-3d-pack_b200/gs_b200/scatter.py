@@ -19,14 +19,11 @@ import ctypes as C
 import torch
 
 from . import _lib
+from ._lib import ptr, stream
 
 _CODE = {torch.float32: _lib.SCATTER_F32, torch.int32: _lib.SCATTER_I32, torch.int64: _lib.SCATTER_I64}
 _SUM_DTYPES = (torch.float32, torch.int32, torch.int64)
 _MEAN_DTYPES = (torch.float32,)
-
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr() if t is not None and t.numel() else None)
 
 
 def _i64(vals):
@@ -92,8 +89,8 @@ class _Call:
         if self.src.numel() == 0:
             return 0 if dim_size is None else int(dim_size)
         rng = torch.empty(2, dtype=torch.int64, device=self.src.device)
-        _lib.check(_lib.lib.gs_b200_scatter_index_range(self.src.dim(), self.shape, self.dim, _ptr(self.index), self.istr,
-                                                        _ptr(rng), _stream()))
+        _lib.check(_lib.lib.gs_b200_scatter_index_range(self.src.dim(), self.shape, self.dim, ptr(self.index), self.istr,
+                                                        ptr(rng), stream()))
         lo, hi = rng.tolist()
         size = hi + 1 if dim_size is None else int(dim_size)
         bad = lo if lo < 0 else (hi if hi >= size else None)
@@ -116,15 +113,11 @@ class _Call:
             raise RuntimeError(f"{self.name}: {_lib.last_error()}")
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         argmax = torch.empty(out.shape, dtype=torch.int64, device=dev) if op == _lib.SCATTER_MAX else None
-        _lib.check(_lib.lib.gs_b200_scatter_forward(op, code, nd, self.shape, self.dim, self.dim_size, _ptr(src),
-                                                    _i64(list(src.stride())), _ptr(self.index), self.istr, _ptr(out),
-                                                    _i64(list(out.stride())), int(has_out), _ptr(argmax), _ptr(scratch),
-                                                    _stream()))
+        _lib.check(_lib.lib.gs_b200_scatter_forward(op, code, nd, self.shape, self.dim, self.dim_size, ptr(src),
+                                                    _i64(list(src.stride())), ptr(self.index), self.istr, ptr(out),
+                                                    _i64(list(out.stride())), int(has_out), ptr(argmax), ptr(scratch),
+                                                    stream()))
         return out, argmax, scratch
-
-
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _backward(op, call, grad, argmax, scratch, want_out):
@@ -133,9 +126,9 @@ def _backward(op, call, grad, argmax, scratch, want_out):
     gout = None
     if want_out and op == _lib.SCATTER_MEAN:
         gout = torch.empty(grad.shape, dtype=torch.float32, device=call.device)
-    _lib.check(_lib.lib.gs_b200_scatter_backward(op, len(call.src_shape), call.shape, call.dim, call.dim_size, _ptr(call.index),
-                                                 call.istr, _ptr(grad), _i64(list(grad.stride())), _ptr(argmax),
-                                                 _ptr(scratch), _ptr(gsrc), _ptr(gout), _stream()))
+    _lib.check(_lib.lib.gs_b200_scatter_backward(op, len(call.src_shape), call.shape, call.dim, call.dim_size, ptr(call.index),
+                                                 call.istr, ptr(grad), _i64(list(grad.stride())), ptr(argmax),
+                                                 ptr(scratch), ptr(gsrc), ptr(gout), stream()))
     if want_out and op == _lib.SCATTER_SUM:
         gout = grad
     return gsrc, gout

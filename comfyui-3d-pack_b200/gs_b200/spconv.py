@@ -17,16 +17,9 @@ import ctypes as C
 import torch
 
 from . import _lib
+from ._lib import ptr, stream
 
 _DTYPES = {torch.float32: _lib.SPCONV_F32, torch.float16: _lib.SPCONV_F16}
-
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr() if t is not None and t.numel() else None)
-
-
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _cuda(name, arg, t):
@@ -95,9 +88,9 @@ def build_map(indices, spatial_shape, batch_size, kernel_size=3):
             if nbytes == 0:
                 raise RuntimeError(f"gs_b200: {_lib.last_error()}")
             scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-            _lib.check(_lib.lib.gs_b200_spconv_build_map(N, B, X, Y, Z, _ptr(idx), _ptr(m.nbr), _ptr(m.mask),
-                                                         _ptr(m.sorted_keys), _ptr(m.sorted_rows), _ptr(scratch),
-                                                         _stream()))
+            _lib.check(_lib.lib.gs_b200_spconv_build_map(N, B, X, Y, Z, ptr(idx), ptr(m.nbr), ptr(m.mask),
+                                                         ptr(m.sorted_keys), ptr(m.sorted_rows), ptr(scratch),
+                                                         stream()))
     return m
 
 
@@ -139,9 +132,9 @@ class SubMConvFunction(torch.autograd.Function):
         with torch.cuda.device(dev):
             out = torch.empty(N, Cout, dtype=features.dtype, device=dev)
             if N:
-                _lib.check(_lib.lib.gs_b200_spconv_forward(dt, N, Cin, Cout, k, _ptr(features), _ptr(nmap.nbr),
-                                                           _ptr(nmap.mask), _ptr(weight), _ptr(bias), _ptr(out),
-                                                           _stream()))
+                _lib.check(_lib.lib.gs_b200_spconv_forward(dt, N, Cin, Cout, k, ptr(features), ptr(nmap.nbr),
+                                                           ptr(nmap.mask), ptr(weight), ptr(bias), ptr(out),
+                                                           stream()))
         ctx.save_for_backward(features, weight)
         ctx.nmap, ctx.dt, ctx.has_bias = nmap, dt, bias is not None
         return out
@@ -164,17 +157,17 @@ class SubMConvFunction(torch.autograd.Function):
             scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             if need_x:
                 gx = torch.empty(N, Cin, dtype=features.dtype, device=dev)
-                _lib.check(_lib.lib.gs_b200_spconv_dgrad(dt, N, Cin, Cout, k, _ptr(grad_out), _ptr(nmap.nbr),
-                                                         _ptr(nmap.mask), _ptr(nmap.sorted_keys),
-                                                         _ptr(nmap.sorted_rows), _ptr(weight), _ptr(gx),
-                                                         _ptr(scratch), _stream()))
+                _lib.check(_lib.lib.gs_b200_spconv_dgrad(dt, N, Cin, Cout, k, ptr(grad_out), ptr(nmap.nbr),
+                                                         ptr(nmap.mask), ptr(nmap.sorted_keys),
+                                                         ptr(nmap.sorted_rows), ptr(weight), ptr(gx),
+                                                         ptr(scratch), stream()))
             if need_w or need_b:
                 gw = torch.empty_like(weight) if need_w else None
                 gb = torch.empty(Cout, dtype=weight.dtype, device=dev) if need_b else None
-                _lib.check(_lib.lib.gs_b200_spconv_wgrad(dt, N, Cin, Cout, k, _ptr(features), _ptr(grad_out),
-                                                         _ptr(nmap.nbr), C.c_void_p(gw.data_ptr() if gw is not None else None),
+                _lib.check(_lib.lib.gs_b200_spconv_wgrad(dt, N, Cin, Cout, k, ptr(features), ptr(grad_out),
+                                                         ptr(nmap.nbr), C.c_void_p(gw.data_ptr() if gw is not None else None),
                                                          C.c_void_p(gb.data_ptr() if gb is not None else None),
-                                                         _ptr(scratch), _stream()))
+                                                         ptr(scratch), stream()))
         return gx, gw, gb, None
 
 

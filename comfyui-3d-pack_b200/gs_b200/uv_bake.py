@@ -14,19 +14,11 @@ import name `slangtorch` (comfyui-3d-pack_b200/slangtorch) serves texture_baker.
 - Deviations, where the reference is undefined: a face with a vertex id out of range is skipped; interpolate of a face
   or vertex id out of range gives 0; a region larger than the texture is clipped.
 """
-import ctypes as C
 
 import torch
 
 from . import _lib
-
-
-def _P(t):
-    return C.c_void_p(t.data_ptr() if t is not None and t.numel() else None)
-
-
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+from ._lib import ptr, stream
 
 
 def _cuda(t, what, dtypes):
@@ -86,8 +78,8 @@ def rasterize_into(uv, faces, out, rows, cols, counts=False):
         if nbytes == 0:
             raise ValueError(f"uv_bake: bad sizes (F = {f.shape[0]}, res = {res})")
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=out.device)
-        _lib.check(_lib.lib.dr_b200_uvbake_rasterize(_P(u), u.shape[0], _P(f), f.shape[0], _P(out), res,
-                                                     max(0, int(rows)), max(0, int(cols)), _P(scratch), _stream()))
+        _lib.check(_lib.lib.dr_b200_uvbake_rasterize(ptr(u), u.shape[0], ptr(f), f.shape[0], ptr(out), res,
+                                                     max(0, int(rows)), max(0, int(cols)), ptr(scratch), stream()))
     if counts:
         return out, tuple(int(x) for x in scratch[:12].view(torch.int32).cpu())
     return out
@@ -116,8 +108,8 @@ def interpolate_into(attr, rast, faces, out, rows, cols):
         raise RuntimeError("attr, rast, faces and output must be on one device")
     r = _aligned(r, 16)
     with torch.cuda.device(out.device):
-        _lib.check(_lib.lib.dr_b200_uvbake_interpolate(_P(a), a.shape[0], _P(f), f.shape[0], _P(r), _P(out), res,
-                                                       max(0, int(rows)), max(0, int(cols)), _stream()))
+        _lib.check(_lib.lib.dr_b200_uvbake_interpolate(ptr(a), a.shape[0], ptr(f), f.shape[0], ptr(r), ptr(out), res,
+                                                       max(0, int(rows)), max(0, int(cols)), stream()))
     return out
 
 

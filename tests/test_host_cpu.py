@@ -78,6 +78,47 @@ def test_ctypes_structs_match_header_layout():
     assert ctypes.sizeof(_lib.State) == ss and _lib.State.num_rendered.offset == onr and _lib.State.owned.offset == oo
 
 
+def test_ctypes_binding_is_derived_from_the_headers():
+    """gs_b200._lib binds every function include/*.h declares, with one argtype per declared parameter; a few
+    signatures are pinned by hand (every row of the C -> ctypes mapping), the header constants reach Python, and a
+    by-value type the mapping does not know is refused rather than guessed."""
+    from gs_b200 import _lib
+    declared = {}
+    for h in ("gs_b200.h", "dr_b200.h", "ngp_b200.h"):
+        src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", h)).read(), flags=re.S)
+        for name, params in re.findall(r"\b((?:gs|dr|ngp)_b200_\w+)\s*\(([^()]*)\)\s*;", src):
+            declared[name] = 0 if params.strip() == "void" else params.count(",") + 1
+    bound = {n for n, f in vars(_lib.lib).items() if isinstance(f, _lib.lib._FuncPtr)}
+    assert len(declared) == 100 and bound == set(declared)
+    for name, nparams in declared.items():
+        assert len(getattr(_lib.lib, name).argtypes) == nparams, name
+
+    I, L, F, D, P, S = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double, ctypes.c_void_p, ctypes.c_size_t
+    expected = {
+        "ngp_b200_grid_encode_fwd": (I, (P, L, P, P, I, F, D, I, P, P)),
+        "gs_b200_adam_step": (I, (I, I, P, D, D, F, I, F, P, P, P, P, P)),
+        "gs_b200_sort_scratch_bytes": (S, (L,)),
+        "gs_b200_launch_count": (L, ()),
+        "gs_b200_last_error": (ctypes.c_char_p, ()),
+        "gs_b200_profile_enable": (None, (I,)),
+        "gs_b200_rasterize_forward": (I, (ctypes.POINTER(_lib.View), I, I) + (P,) * 11 +
+                                      (_lib.ALLOC_FN, P, ctypes.POINTER(_lib.State), P)),
+        "gs_b200_step_device_hook": (I, (I, I, I, I, F, P, P, I, I) + (P,) * 9 + (_lib.VIEW_HOOK, P, P, P)),
+        "gs_b200_set_grad_sink": (I, (_lib.GRAD_SINK, P, I)),
+    }
+    for name, (restype, argtypes) in expected.items():
+        fn = getattr(_lib.lib, name)
+        assert (fn.restype, tuple(fn.argtypes)) == (restype, argtypes), name
+
+    assert _lib.SPCONV_MAX_ROWS == (1 << 30) - 1 and _lib.PN2_FPS_ONCHIP_MAX == 16384
+    assert _lib.SCATTER_MAX_DIMS == 8 and _lib.BUF_SCRATCH == 3
+    assert _lib.NSTAGES == len(_lib.STAGE_NAMES) == 9
+
+    assert _lib.prototypes("int32_t gs_b200_x(const uint8_t* x, void* stream);") == {"gs_b200_x": (I, [P, P])}
+    with pytest.raises(ImportError, match="gs_b200_x.*uint8_t"):
+        _lib.prototypes("int32_t gs_b200_x(uint8_t x);")
+
+
 def test_settings_namedtuple_field_order_matches_reference_call_site():
     # main_3DGS_renderer.py:849-862 constructs it by keyword; LGM/TRELLIS too. Order = the package's NamedTuple.
     from diff_gaussian_rasterization import GaussianRasterizationSettings

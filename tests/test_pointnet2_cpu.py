@@ -168,11 +168,12 @@ def test_shim_names():
             fn(0.1, 16)
 
 
-def test_c_abi_exports():
+def test_c_abi_scratch_bytes():
     from gs_b200 import _lib
-    for name in _lib.PN2_EXPORTS:
-        assert getattr(_lib.lib, name)
-    assert name in _lib.EXPORTS
+    sb = _lib.lib.gs_b200_pn2_backward_scratch_bytes
+    assert sb(2, 3, 100, 50, 1) > sb(2, 3, 100, 50, 0) > 0
+    assert sb(1, 1, 0, 1, 0) == 0 and sb(1, 1, 1, -1, 0) == 0
+    assert sb(1, 1, 8, 1 << 32, 0) == 0          # M is int64: 2^32 index entries are refused, not truncated to 0
 
 
 def test_cpu_tensors_and_dtypes_raise_before_gpu_work():

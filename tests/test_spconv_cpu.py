@@ -213,8 +213,9 @@ def test_argument_errors_before_gpu_work():
         sp.SubMConv3d(5, 4, 3)(x)
 
 
-def test_c_abi_exports():
+def test_c_abi_scratch_bytes():
     from gs_b200 import _lib
-    for name in _lib.SPCONV_EXPORTS:
-        assert getattr(_lib.lib, name)
-        assert name in _lib.EXPORTS
+    sb = _lib.lib.gs_b200_spconv_map_scratch_bytes
+    assert sb(_lib.SPCONV_MAX_ROWS) > sb(1000) > 0
+    assert sb(_lib.SPCONV_MAX_ROWS + 1) == 0 and sb(-1) == 0
+    assert sb(1 << 32) == 0                      # N is int64: 2^32 rows are refused, not truncated to 0
