@@ -12,6 +12,7 @@
 // that offset into shared memory; every output is one fixed-order sum, so results have the same bits on every run.
 #include "../../include/gs_b200.h"
 #include "gs_common.cuh"
+#include "mma_sm90.cuh"
 
 #include <cuda_fp16.h>
 #include <algorithm>
@@ -138,25 +139,6 @@ __device__ __forceinline__ int src_row(const Gemm& a, int r, int o) {
 // cp.async ring (16 B copies with zero-fill for absent rows and tails) padded to 40 halves per row so that ldmatrix
 // reads are free of bank conflicts.  VEC = false (Kin not a multiple of 8 or an unaligned base) loads element-wise.
 constexpr int HBM = 64, HBN = 64, HBK = 32, HST = 3, HLD = HBK + 8, HT = 128;
-
-__device__ __forceinline__ void cp_async16(void* dst, const void* src, int bytes) {
-    const uint32_t d = (uint32_t)__cvta_generic_to_shared(dst);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(d), "l"(src), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int n> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(n) : "memory"); }
-
-__device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], const void* p) {
-    const uint32_t a = (uint32_t)__cvta_generic_to_shared(p);
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(a));
-}
-__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
-                 "{%0,%1,%2,%3};"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 
 template <bool VEC>
 __device__ __forceinline__ void load_chunk16(__half* dst, const __half* base, int rowsrc, int c, int lim) {

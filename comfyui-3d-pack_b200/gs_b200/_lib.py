@@ -87,20 +87,37 @@ if not os.path.exists(LIB_PATH):
 lib = C.CDLL(LIB_PATH)
 
 
+def _bind_header(handle, h):
+    """Bind every function header `h` (a name under include/, or a path) declares on `handle`; returns the header's
+    constants."""
+    path = os.path.join(_INCLUDE, h)
+    if not os.path.exists(path):
+        raise ImportError(f"{path} is missing: gs_b200 binds its libraries from the headers under include/.")
+    with open(path) as f:
+        src = f.read()
+    for name, (restype, argtypes) in prototypes(src).items():
+        fn = getattr(handle, name)
+        fn.restype, fn.argtypes = restype, argtypes
+    return constants(src)
+
+
 def _bind():
     for h in _HEADERS:
-        path = os.path.join(_INCLUDE, h)
-        if not os.path.exists(path):
-            raise ImportError(f"{path} is missing: gs_b200 binds libgs_b200.so from the headers under include/.")
-        with open(path) as f:
-            src = f.read()
-        for name, (restype, argtypes) in prototypes(src).items():
-            fn = getattr(lib, name)
-            fn.restype, fn.argtypes = restype, argtypes
-        globals().update(constants(src))
+        globals().update(_bind_header(lib, h))
 
 
 _bind()
+
+
+def companion(so_name, header):
+    """(handle, constants) of a library built beside libgs_b200.so and linked against it (csrc/build.sh), bound from
+    its own header (a path) in the same way.  Raises ImportError when it has not been built."""
+    path = os.path.join(_HERE, so_name)
+    if not os.path.exists(path):
+        raise ImportError(f"{path} is missing: the sm_90a CUDA library has not been built. "
+                          "Run `python __graft_entry__.py` (or comfyui-3d-pack_b200/csrc/build.sh). There is no CPU fallback.")
+    handle = C.CDLL(path)
+    return handle, _bind_header(handle, header)
 
 
 def last_error() -> str:
