@@ -19,7 +19,12 @@ done
 # attention (flash_attn drop-in): its own library, linked against libgs_b200.so for the error and launch counters
 mkdir -p build/attn
 $NVCC $COMMON -c gs_attn.cu -o build/attn/gs_attn.o & pids+=($!)
+# point rasterizer (pytorch3d PointsRasterizer / points_projection drop-in): a companion library in the same way;
+# no FMA contraction (bit-exact projection, pixel centres and distances vs the oracle)
+mkdir -p build/pts
+$NVCC $COMMON -fmad=false -c pts_raster.cu -o build/pts/pts_raster.o & pids+=($!)
 for p in "${pids[@]}"; do wait $p; done
 $NVCC -shared $ARCH -o ../gs_b200/libgs_b200.so build/*.o -lcudart
 $NVCC -shared $ARCH -o ../gs_b200/libgs_attn.so build/attn/gs_attn.o -L../gs_b200 -lgs_b200 -lcudart -Xlinker -rpath -Xlinker '$ORIGIN'
-echo "built $(realpath ../gs_b200/libgs_b200.so) $(realpath ../gs_b200/libgs_attn.so)"
+$NVCC -shared $ARCH -o ../gs_b200/libgs_pts.so build/pts/pts_raster.o -L../gs_b200 -lgs_b200 -lcudart -Xlinker -rpath -Xlinker '$ORIGIN'
+echo "built $(realpath ../gs_b200/libgs_b200.so) $(realpath ../gs_b200/libgs_attn.so) $(realpath ../gs_b200/libgs_pts.so)"

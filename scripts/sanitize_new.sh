@@ -139,3 +139,33 @@ for tool in memcheck racecheck; do
   timeout 1200 compute-sanitizer --tool $tool --error-exitcode 9 --launch-timeout 0 python /tmp/sp_case.py 2>&1 | tail -6
   echo "sp $tool rc=$?"
 done
+
+# point rasterizer and points_projection (pts_raster.cu): K = 1, 2 and 8, ragged clouds with an empty one, a shared
+# camera, points behind and on the camera plane, the lift from strided features and its backward; memcheck and racecheck
+cat > /tmp/pts_case.py <<'PY'
+import sys, os
+ROOT = os.getcwd(); sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "comfyui-3d-pack_b200"))
+import torch
+from gs_b200 import points as P
+dev = torch.device("cuda:0")
+g = torch.Generator(device=dev).manual_seed(0)
+R = torch.eye(3, device=dev)[None].repeat(3, 1, 1); T = torch.tensor([[0.0, 0.0, 2.0]], device=dev).repeat(3, 1)
+Km = torch.tensor([[[30.0, 0, 40], [0, 30, 30], [0, 0, 1]]], device=dev).repeat(3, 1, 1)
+cams = P.cameras_from_opencv_projection(R, T, Km, torch.tensor([[60, 80]] * 3, device=dev))
+clouds = [torch.rand(900, 3, generator=g, device=dev) * 2 - 1, torch.zeros(0, 3, device=dev), torch.rand(50, 3, generator=g, device=dev) * 6 - 3]
+for K in (1, 2, 8):
+    fr = P.PointsRasterizer(cams, P.PointsRasterizationSettings((60, 80), 0.05, K))(P.Pointclouds(clouds))
+    fr1 = P.PointsRasterizer(P.cameras_from_opencv_projection(R[:1], T[:1], Km[:1], torch.tensor([[60, 80]], device=dev)),
+                             P.PointsRasterizationSettings((60, 80), 0.05, K))(P.Pointclouds(clouds))
+pts = torch.rand(2, 2000, 3, generator=g, device=dev) - 0.5
+c2w = torch.eye(4, device=dev)[None].repeat(2, 1, 1); c2w[:, 2, 3] = -2.0
+f = torch.randn(2, 40, 7, 60, generator=g, device=dev).permute(0, 3, 2, 1).requires_grad_(True)
+Kf = torch.tensor([[[12.0, 0, 20], [0, 12, 3.5], [0, 0, 1]]], device=dev).repeat(2, 1, 1)
+for K in (1, 3):
+    P.points_projection(pts, c2w, Kf, f, 0.03, K).sum().backward()
+torch.cuda.synchronize(); print("pts ok", int((fr.idx >= 0).sum()), float(f.grad.abs().sum()))
+PY
+for tool in memcheck racecheck; do
+  timeout 1200 compute-sanitizer --tool $tool --error-exitcode 9 --launch-timeout 0 python /tmp/pts_case.py 2>&1 | tail -6
+  echo "pts $tool rc=$?"
+done
