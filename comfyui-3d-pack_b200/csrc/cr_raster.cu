@@ -18,6 +18,7 @@
 // the order written, as gcc evaluates the reference's CPU path.
 #include <type_traits>
 
+#include "../../include/dr_b200.h"
 #include "gs_common.cuh"
 
 namespace {
@@ -272,12 +273,38 @@ void interp_launch(const float* col, int NV, int C, const void* fid, const float
                                                                dbary, contrib, cidx);
 }
 
+// both interpolation entry points: the forward when g is NULL, else the backward
+int interpolate(const float* col, int NV, int C, const void* fid, int fid_f32, const float* bary, const void* tri,
+                int tri_i64, int NF, int npix, const float* g, float* out, float* dbary, float* contrib, long long* cidx,
+                cudaStream_t s) {
+    if (npix == 0) return 0;
+    if (fid_f32) {
+        if (tri_i64) interp_launch<float, long long>(col, NV, C, fid, bary, tri, NF, npix, g, out, dbary, contrib, cidx, s);
+        else interp_launch<float, int32_t>(col, NV, C, fid, bary, tri, NF, npix, g, out, dbary, contrib, cidx, s);
+    } else {
+        if (tri_i64) interp_launch<int32_t, long long>(col, NV, C, fid, bary, tri, NF, npix, g, out, dbary, contrib, cidx, s);
+        else interp_launch<int32_t, int32_t>(col, NV, C, fid, bary, tri, NF, npix, g, out, dbary, contrib, cidx, s);
+    }
+    gs_count_launches(1);
+    GS_CUDA_CHECK(cudaGetLastError());
+    return 0;
+}
+
 }  // namespace
 
-size_t cr_scratch_bytes(int F, int H, int W) { return (size_t)H * W * 8 + 256 + (size_t)F * 8; }
+extern "C" {
 
-int cr_launch_rasterize(const float* V, int NV, const int32_t* T, int NF, const float* D, int H, int W, float trunc,
-                        int32_t* findices, float* bary, void* scratch, cudaStream_t s) {
+size_t dr_b200_cr_scratch_bytes(int32_t F, int32_t H, int32_t W) {
+    return (F < 0 || H <= 0 || W <= 0) ? 0 : (size_t)H * W * 8 + 256 + (size_t)F * 8;
+}
+
+int32_t dr_b200_cr_rasterize(const float* V, int32_t NV, const int32_t* T, int32_t NF, const float* D, int32_t H, int32_t W,
+                             float trunc, int32_t* findices, float* bary, void* scratch, void* stream) {
+    GS_REQ(NV >= 0 && NF >= 0 && H > 0 && W > 0, "bad sizes");
+    GS_REQ(H <= (1 << 24) && W <= (1 << 24) && (int64_t)H * W <= INT32_MAX / 3, "image too large");
+    GS_REQ(findices && bary && scratch && (NF == 0 || (V && T)), "NULL pointer");
+    GS_REQ(((size_t)V & 15) == 0, "pos must be 16-byte aligned");
+    const cudaStream_t s = (cudaStream_t)stream;
     const size_t npix = (size_t)H * W;
     unsigned long long* zbuf = (unsigned long long*)scratch;
     uint32_t* counts = (uint32_t*)((char*)scratch + npix * 8);
@@ -295,18 +322,24 @@ int cr_launch_rasterize(const float* V, int NV, const int32_t* T, int NF, const 
     return 0;
 }
 
-int cr_launch_interpolate(const float* col, int NV, int C, const void* fid, int fid_f32, const float* bary, const void* tri,
-                          int tri_i64, int NF, int npix, const float* g, float* out, float* dbary, float* contrib,
-                          long long* cidx, cudaStream_t s) {
-    if (npix == 0) return 0;
-    if (fid_f32) {
-        if (tri_i64) interp_launch<float, long long>(col, NV, C, fid, bary, tri, NF, npix, g, out, dbary, contrib, cidx, s);
-        else interp_launch<float, int32_t>(col, NV, C, fid, bary, tri, NF, npix, g, out, dbary, contrib, cidx, s);
-    } else {
-        if (tri_i64) interp_launch<int32_t, long long>(col, NV, C, fid, bary, tri, NF, npix, g, out, dbary, contrib, cidx, s);
-        else interp_launch<int32_t, int32_t>(col, NV, C, fid, bary, tri, NF, npix, g, out, dbary, contrib, cidx, s);
-    }
-    gs_count_launches(1);
-    GS_CUDA_CHECK(cudaGetLastError());
-    return 0;
+int32_t dr_b200_cr_interpolate_fwd(const float* col, int32_t V, int32_t C, const void* findices, int32_t findices_f32,
+                                   const float* barycentric, const void* tri, int32_t tri_i64, int32_t F, int32_t npix,
+                                   float* out, void* stream) {
+    GS_REQ(V >= 0 && C > 0 && F >= 0 && npix >= 0 && (int64_t)npix * 3 <= INT32_MAX, "bad sizes");
+    GS_REQ(npix == 0 || (findices && barycentric && out && (F == 0 || tri) && (V == 0 || col)), "NULL pointer");
+    return interpolate(col, V, C, findices, findices_f32, barycentric, tri, tri_i64, F, npix, nullptr, out, nullptr,
+                       nullptr, nullptr, (cudaStream_t)stream);
 }
+
+int32_t dr_b200_cr_interpolate_bwd(const float* col, int32_t V, int32_t C, const void* findices, int32_t findices_f32,
+                                   const float* barycentric, const void* tri, int32_t tri_i64, int32_t F, int32_t npix,
+                                   const float* grad_out, float* grad_barycentric, float* contrib, int64_t* contrib_index,
+                                   void* stream) {
+    GS_REQ(V >= 0 && C > 0 && F >= 0 && npix >= 0 && (int64_t)npix * 3 <= INT32_MAX, "bad sizes");
+    GS_REQ(npix == 0 || (findices && barycentric && grad_out && (F == 0 || tri) && (V == 0 || col)), "NULL pointer");
+    GS_REQ((contrib == nullptr) == (contrib_index == nullptr), "contrib and contrib_index go together");
+    return interpolate(col, V, C, findices, findices_f32, barycentric, tri, tri_i64, F, npix, grad_out, nullptr,
+                       grad_barycentric, contrib, (long long*)contrib_index, (cudaStream_t)stream);
+}
+
+}  // extern "C"

@@ -6,6 +6,7 @@
 // mesh_utils.py:534).  All four are one-pass, per-pixel, HBM/L2-bound kernels: full-frame buffers are read
 // once with 128-bit accesses where the layout allows, vertex attributes / texels are gathered through L2,
 // gradients to shared data (attributes, texels, vertex positions) leave as red.global.add.
+#include "../../include/dr_b200.h"
 #include "gs_common.cuh"
 
 namespace {
@@ -324,8 +325,15 @@ antialias_bwd_kernel(const float* __restrict__ color, const float4* __restrict__
 
 #define DR_GRID(n) (unsigned)(((n) + 255) / 256), 256
 
-int dr_launch_interpolate_fwd(const float* attr, int attr_B, const float* rast, const int32_t* tri, const float* rast_db,
-                              int B, int V, int F, int H, int W, int A, float* out, float* out_da, cudaStream_t s) {
+extern "C" {
+
+int32_t dr_b200_interpolate_fwd(const float* attr, int32_t attr_B, const float* rast, const int32_t* tri, const float* rast_db,
+                                int32_t B, int32_t V, int32_t F, int32_t H, int32_t W, int32_t A, float* out, float* out_da,
+                                void* stream) {
+    GS_REQ(attr && rast && tri && out, "NULL pointer");
+    GS_REQ(attr_B == 1 || attr_B == B, "attr batch must be 1 or B");
+    GS_REQ((out_da == nullptr) || (rast_db != nullptr), "out_da needs rast_db");
+    const cudaStream_t s = (cudaStream_t)stream;
     const size_t npix = (size_t)B * H * W;
     if (npix == 0) return 0;
     interpolate_fwd_kernel<<<DR_GRID(npix), 0, s>>>(attr, attr_B, (const float4*)rast, tri, (const float4*)rast_db, B, V, H, W, A, out, out_da);
@@ -333,9 +341,12 @@ int dr_launch_interpolate_fwd(const float* attr, int attr_B, const float* rast, 
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
 }
-int dr_launch_interpolate_bwd(const float* attr, int attr_B, const float* rast, const int32_t* tri, const float* rast_db,
-                              int B, int V, int F, int H, int W, int A, const float* g_out, const float* g_da,
-                              float* d_attr, float* d_rast, float* d_db, cudaStream_t s) {
+int32_t dr_b200_interpolate_bwd(const float* attr, int32_t attr_B, const float* rast, const int32_t* tri, const float* rast_db,
+                                int32_t B, int32_t V, int32_t F, int32_t H, int32_t W, int32_t A, const float* g_out,
+                                const float* g_da, float* d_attr, float* d_rast, float* d_db, void* stream) {
+    GS_REQ(attr && rast && tri && g_out && d_attr && d_rast, "NULL pointer");
+    GS_REQ((g_da == nullptr) || (rast_db != nullptr), "dL_dout_da needs rast_db");
+    const cudaStream_t s = (cudaStream_t)stream;
     const size_t npix = (size_t)B * H * W;
     if (npix == 0) return 0;
     interpolate_bwd_kernel<<<DR_GRID(npix), 0, s>>>(attr, attr_B, (const float4*)rast, tri, (const float4*)rast_db, B, V, H, W, A,
@@ -344,8 +355,11 @@ int dr_launch_interpolate_bwd(const float* attr, int attr_B, const float* rast, 
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
 }
-int dr_launch_texture_fwd(const float* tex, int tex_B, int Ht, int Wt, int C, const float* uv, int B, int H, int W,
-                          int boundary, float* out, cudaStream_t s) {
+int32_t dr_b200_texture_fwd(const float* tex, int32_t tex_B, int32_t Ht, int32_t Wt, int32_t C, const float* uv, int32_t B,
+                            int32_t H, int32_t W, int32_t boundary, float* out, void* stream) {
+    GS_REQ(tex && uv && out && Ht > 0 && Wt > 0 && C > 0, "bad argument");
+    GS_REQ(tex_B == 1 || tex_B == B, "tex batch must be 1 or B");
+    const cudaStream_t s = (cudaStream_t)stream;
     const size_t npix = (size_t)B * H * W;
     if (npix == 0) return 0;
     texture_fwd_kernel<<<DR_GRID(npix), 0, s>>>(tex, tex_B, Ht, Wt, C, (const float2*)uv, B, H, W, boundary, out);
@@ -353,8 +367,11 @@ int dr_launch_texture_fwd(const float* tex, int tex_B, int Ht, int Wt, int C, co
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
 }
-int dr_launch_texture_bwd(const float* tex, int tex_B, int Ht, int Wt, int C, const float* uv, int B, int H, int W,
-                          int boundary, const float* g_out, float* d_tex, float* d_uv, cudaStream_t s) {
+int32_t dr_b200_texture_bwd(const float* tex, int32_t tex_B, int32_t Ht, int32_t Wt, int32_t C, const float* uv, int32_t B,
+                            int32_t H, int32_t W, int32_t boundary, const float* g_out, float* d_tex, float* d_uv,
+                            void* stream) {
+    GS_REQ(tex && uv && g_out && d_tex && d_uv, "NULL pointer");
+    const cudaStream_t s = (cudaStream_t)stream;
     const size_t npix = (size_t)B * H * W;
     if (npix == 0) return 0;
     texture_bwd_kernel<<<DR_GRID(npix), 0, s>>>(tex, tex_B, Ht, Wt, C, (const float2*)uv, B, H, W, boundary, g_out, d_tex, (float2*)d_uv);
@@ -363,12 +380,14 @@ int dr_launch_texture_bwd(const float* tex, int tex_B, int Ht, int Wt, int C, co
     return 0;
 }
 
-size_t dr_topology_scratch_bytes(int F) {
+size_t dr_b200_topology_scratch_bytes(int32_t F) {
     const size_t n = (size_t)3 * F;
     return ((n * 4 + 255) & ~(size_t)255) * 4 + gs_sort_scratch_bytes((int64_t)n) + 256;
 }
 
-int dr_launch_edge_opposites(const int32_t* tri, int F, int V, int32_t* opp, void* scratch, cudaStream_t s) {
+int32_t dr_b200_edge_opposites(const int32_t* tri, int32_t F, int32_t V, int32_t* opp, void* scratch, void* stream) {
+    GS_REQ(F == 0 || (tri && opp && scratch), "NULL pointer");
+    const cudaStream_t s = (cudaStream_t)stream;
     if (F <= 0) return 0;
     const int n = 3 * F;
     const size_t stride = ((size_t)n * 4 + 255) & ~(size_t)255;
@@ -392,8 +411,10 @@ int dr_launch_edge_opposites(const int32_t* tri, int F, int V, int32_t* opp, voi
     return 0;
 }
 
-int dr_launch_antialias_fwd(const float* color, const float* rast, const float* pos, const int32_t* tri, const int32_t* opp,
-                            int B, int V, int F, int H, int W, int C, float* out, cudaStream_t s) {
+int32_t dr_b200_antialias_fwd(const float* color, const float* rast, const float* pos, const int32_t* tri, const int32_t* opp,
+                              int32_t B, int32_t V, int32_t F, int32_t H, int32_t W, int32_t C, float* out, void* stream) {
+    GS_REQ(color && rast && out && (F == 0 || (pos && tri && opp)), "NULL pointer");
+    const cudaStream_t s = (cudaStream_t)stream;
     const size_t npix = (size_t)B * H * W;
     if (npix == 0) return 0;
     GS_CUDA_CHECK(cudaMemcpyAsync(out, color, npix * C * 4, cudaMemcpyDeviceToDevice, s));
@@ -404,9 +425,11 @@ int dr_launch_antialias_fwd(const float* color, const float* rast, const float* 
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
 }
-int dr_launch_antialias_bwd(const float* color, const float* rast, const float* pos, const int32_t* tri, const int32_t* opp,
-                            int B, int V, int F, int H, int W, int C, const float* g_out, float* d_color, float* d_pos,
-                            cudaStream_t s) {
+int32_t dr_b200_antialias_bwd(const float* color, const float* rast, const float* pos, const int32_t* tri, const int32_t* opp,
+                              int32_t B, int32_t V, int32_t F, int32_t H, int32_t W, int32_t C, const float* g_out,
+                              float* d_color, float* d_pos, void* stream) {
+    GS_REQ(color && rast && g_out && d_color && (F == 0 || (pos && tri && opp && d_pos)), "NULL pointer");
+    const cudaStream_t s = (cudaStream_t)stream;
     const size_t npix = (size_t)B * H * W;
     if (npix == 0) return 0;
     GS_CUDA_CHECK(cudaMemcpyAsync(d_color, g_out, npix * C * 4, cudaMemcpyDeviceToDevice, s));
@@ -417,3 +440,5 @@ int dr_launch_antialias_bwd(const float* color, const float* rast, const float* 
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
 }
+
+}  // extern "C"

@@ -15,6 +15,7 @@
 // zeros, are deferred to a second pass that decides them exactly.
 // THIS TU IS COMPILED WITH -fmad=false: z/w (and u, v) use the exact fp32 operation order of oracle/dr_oracle.py, so
 // triangle ids are bit-exact against the oracle.
+#include "../../include/dr_b200.h"
 #include "gs_common.cuh"
 
 namespace {
@@ -367,12 +368,18 @@ raster_backward_kernel(const float4* __restrict__ pos, const int32_t* __restrict
 // pixels within rounding of an edge); beyond it the overflow pass stays correct, only slower
 static size_t deferred_cap(int B, int F) { return (size_t)2 * B * F + 4096; }
 
-size_t dr_rasterize_scratch_bytes(int B, int F, int H, int W) {
+extern "C" {
+
+size_t dr_b200_rasterize_scratch_bytes(int32_t B, int32_t F, int32_t H, int32_t W) {
     return (size_t)B * H * W * 8 + 256 + deferred_cap(B, F) * 8 + (size_t)B * F * 4;
 }
 
-int dr_launch_rasterize_fwd(const float* pos, const int32_t* tri, int B, int V, int F, int H, int W, float* rast,
-                            float* rast_db, void* scratch, cudaStream_t s) {
+int32_t dr_b200_rasterize_fwd(const float* pos, const int32_t* tri, int32_t B, int32_t V, int32_t F, int32_t H, int32_t W,
+                              float* rast, float* rast_db, void* scratch, void* stream) {
+    GS_REQ(B >= 0 && V >= 0 && F >= 0 && H > 0 && W > 0, "bad sizes");
+    GS_REQ(rast && rast_db && scratch && (F == 0 || (pos && tri)), "NULL pointer");
+    GS_REQ(((size_t)pos & 15) == 0 && ((size_t)rast & 15) == 0 && ((size_t)rast_db & 15) == 0, "pos/rast must be 16-byte aligned");
+    const cudaStream_t s = (cudaStream_t)stream;
     if (B <= 0 || H <= 0 || W <= 0) return 0;
     const size_t npix = (size_t)B * H * W;
     unsigned long long* zbuf = (unsigned long long*)scratch;
@@ -400,8 +407,10 @@ int dr_launch_rasterize_fwd(const float* pos, const int32_t* tri, int B, int V, 
     return 0;
 }
 
-int dr_launch_rasterize_bwd(const float* pos, const int32_t* tri, int B, int V, int F, int H, int W, const float* rast,
-                            const float* dL_drast, float* dL_dpos, cudaStream_t s) {
+int32_t dr_b200_rasterize_bwd(const float* pos, const int32_t* tri, int32_t B, int32_t V, int32_t F, int32_t H, int32_t W,
+                              const float* rast, const float* dL_drast, float* dL_dpos, void* stream) {
+    GS_REQ(pos && tri && rast && dL_drast && dL_dpos, "NULL pointer");
+    const cudaStream_t s = (cudaStream_t)stream;
     if (B <= 0 || F <= 0) return 0;
     const size_t npix = (size_t)B * H * W;
     const float sx = (float)(2.0 / (double)W), sy = (float)(2.0 / (double)H);
@@ -411,3 +420,5 @@ int dr_launch_rasterize_bwd(const float* pos, const int32_t* tri, int B, int V, 
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
 }
+
+}  // extern "C"

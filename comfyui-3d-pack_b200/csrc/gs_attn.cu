@@ -1,5 +1,5 @@
 // Variable-length multi-head attention forward (flash_attn's varlen / dense entry points, head dim 64, fp16 and bf16)
-// on the GPU (csrc/gs_b200_attn.h, libgs_attn.so): a FlashAttention-2-style kernel on mma.sync tensor cores.
+// on the GPU (include/gs_b200_attn.h): a FlashAttention-2-style kernel on mma.sync tensor cores.
 //
 // A CTA owns 64 query rows (4 warps x 16) of one (sequence, head) and streams the sequence's keys and values in 64-row
 // tiles through a double-buffered cp.async ring; rows past the sequence's end are zero-filled.  Per tile, S = Q.K^T
@@ -8,7 +8,7 @@
 // to the input dtype in registers and reused as the A fragment of O += P.V, with V read by ldmatrix.trans.  At the
 // end O is divided by l once (0 for an empty key set) and rounded once.  Every sum has a fixed order that depends only
 // on the row's position in its sequence, so every output has the same bits on every run, whatever the batch around it.
-#include "gs_b200_attn.h"
+#include "../../include/gs_b200_attn.h"
 #include "gs_common.cuh"
 #include "mma_sm90.cuh"
 

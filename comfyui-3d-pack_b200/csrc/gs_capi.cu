@@ -222,17 +222,6 @@ int32_t gs_b200_profile_read(float* ms_out, int32_t* calls_out) {
 }
 const char* gs_b200_last_error(void) { return g_err; }
 
-size_t gs_b200_sort_scratch_bytes(int64_t n) { return gs_sort_scratch_bytes(n); }
-
-int32_t gs_b200_sort_pairs_u32(uint32_t* keys, uint32_t* keys_alt, uint32_t* vals, uint32_t* vals_alt, int64_t n,
-                               int32_t begin_bit, int32_t end_bit, void* scratch, int32_t* result_in_alt,
-                               void* stream) {
-    int r = 0;
-    int rc = gs_sort_pairs_u32(keys, keys_alt, vals, vals_alt, n, begin_bit, end_bit, scratch, &r, (cudaStream_t)stream);
-    if (result_in_alt) *result_in_alt = r;
-    return rc;
-}
-
 // ---- binning of nv views ----------------------------------------------------------------------------------
 // Inputs are the preprocess's [nv][N] arrays (one view: the single-view entries; a chunk of views: the multi-view
 // step).  Every stage is one launch (or one launch per digit pass) over all nv views.
@@ -548,10 +537,6 @@ int32_t gs_b200_debug_preprocess_backward_multi(int32_t V, int32_t H, int32_t W,
                                 sg + (size_t)v0 * N, gm, g2, gsh, gop, gsc, grt, s, [](int, int) {})) return 1;
     }
     return 0;
-}
-
-int32_t gs_b200_knn_mean_dist2(const float* points, int32_t N, float* out, void* stream_) {
-    return gs_launch_knn(points, N, out, (cudaStream_t)stream_);
 }
 
 // ---------------------------------------------------------------------------------
@@ -1136,25 +1121,6 @@ int32_t gs_b200_step_host_dev_grads(int32_t V, int32_t H, int32_t W, int32_t sh_
     return step_host_impl(V, H, W, sh_degree, scale_modifier, views_host, N, M, means3D_host, shs_host,
                           opacities_host, scales_host, rotations_host, dL_dout_host, nullptr, grads_dev,
                           images_host, num_rendered_out, stream_);
-}
-
-// ---- optimisation-step kernels (gs_train.cu) -------------------------------------------------------------
-
-int32_t gs_b200_activate(int32_t N, const float* raw_opacities, const float* raw_scales, const float* raw_rotations,
-                         float* opacities, float* scales, float* rotations, void* stream_) {
-    if (N > 0 && (!raw_opacities || !raw_scales || !raw_rotations || !opacities || !scales || !rotations)) { gs_set_error("activate: NULL"); return 1; }
-    return gs_launch_activate(N, raw_opacities, raw_scales, raw_rotations, opacities, scales, rotations, (cudaStream_t)stream_);
-}
-int32_t gs_b200_adam_step(int32_t N, int32_t M, const float* lrs6_host, double beta1, double beta2, float eps, int32_t step,
-                          float grad_scale, const float* grads_packed, float* params_packed, float* exp_avg,
-                          float* exp_avg_sq, void* stream_) {
-    if (!lrs6_host || step < 1 || (N > 0 && (!grads_packed || !params_packed || !exp_avg || !exp_avg_sq))) { gs_set_error("adam_step: bad argument"); return 1; }
-    return gs_launch_adam(N, M, lrs6_host, beta1, beta2, eps, step, grad_scale, grads_packed, params_packed, exp_avg, exp_avg_sq, (cudaStream_t)stream_);
-}
-int32_t gs_b200_densify_stats(int32_t N, const float* dL_dmeans2D, const int32_t* radii, float* xyz_gradient_accum,
-                              float* denom, float* max_radii2D, void* stream_) {
-    if (N > 0 && (!dL_dmeans2D || !radii || !xyz_gradient_accum || !denom || !max_radii2D)) { gs_set_error("densify_stats: NULL"); return 1; }
-    return gs_launch_densify_stats(N, dL_dmeans2D, radii, xyz_gradient_accum, denom, max_radii2D, (cudaStream_t)stream_);
 }
 
 }  // extern "C"

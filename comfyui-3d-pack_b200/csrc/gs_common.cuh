@@ -181,6 +181,9 @@ __device__ __forceinline__ void gs_stage_rows_out(const float* __restrict__ s, f
 void gs_set_error(const char* fmt, ...);
 void gs_count_launches(int n);     // instrumentation: kernels launched by this library
 
+// argument check of a C entry point: on failure, "<entry point>: <msg>" becomes the last error and the call returns 1
+#define GS_REQ(cond, msg) do { if (!(cond)) { gs_set_error("%s: %s", __func__, msg); return 1; } } while (0)
+
 // ---- launchers implemented in the .cu files --------------------------------
 int gs_launch_preprocess(const ViewArgs& va, int N, int M, const float* means3D, const float* shs,
                          const float* colors_precomp, const float* opacities, const float* scales,
@@ -215,10 +218,6 @@ int gs_launch_preprocess_backward_multi(const float* views_dev, int V, int W, in
 size_t gs_image_loss_scratch_bytes(int H, int W);
 int gs_launch_image_loss(int H, int W, const float* img, const float* ref, const float* mask, float lambda_ssim,
                          float lambda_alpha, float scale, float* dL, float* loss_out, void* scratch, cudaStream_t s);
-
-int gs_launch_activate(int, const float*, const float*, const float*, float*, float*, float*, cudaStream_t);
-int gs_launch_adam(int, int, const float*, double, double, float, int, float, const float*, float*, float*, float*, cudaStream_t);
-int gs_launch_densify_stats(int, const float*, const int32_t*, float*, float*, float*, cudaStream_t);
 
 // Segmented sort (gs_sort.cu): n segments [off[i], off[i+1]) of one key array, sorted independently in one
 // launch per digit pass.  The multi-view step sorts the depth keys and the tile keys of all views of a chunk so.
@@ -267,4 +266,3 @@ int gs_launch_render_backward(const ViewArgs& va, const SplatRec* recs, const ui
                               SplatGrad* sg, cudaStream_t s);
 int gs_launch_sorted_keys(const SplatRec* recs, const uint32_t* point_list, const uint32_t* tile_keys, int64_t P,
                           uint64_t* keys_out, cudaStream_t s);
-int gs_launch_knn(const float* points, int N, float* out, cudaStream_t s);

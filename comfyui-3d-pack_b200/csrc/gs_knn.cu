@@ -10,6 +10,7 @@
 //                     with the library's radix sort, then per point ring-by-ring search of the surrounding cells
 //                     until the third-best distance is inside the searched block ((ring * cell)^2 bound) — exact,
 //                     O(N) for non-degenerate clouds.
+#include "../../include/gs_b200.h"
 #include "gs_common.cuh"
 #include <algorithm>
 #include <cmath>
@@ -182,7 +183,8 @@ __global__ void __launch_bounds__(128) knn_search_kernel(const float4* __restric
 }
 }  // namespace
 
-int gs_launch_knn(const float* points, int N, float* out, cudaStream_t s) {
+extern "C" int32_t gs_b200_knn_mean_dist2(const float* points, int32_t N, float* out, void* stream) {
+    const cudaStream_t s = (cudaStream_t)stream;
     if (N <= 0) return 0;
     if (!points || !out) { gs_set_error("knn: NULL"); return 1; }
     if (N < 8192) {

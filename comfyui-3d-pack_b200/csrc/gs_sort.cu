@@ -12,6 +12,7 @@
 //
 // The sort is STABLE (ties keep input order), which the tile/depth/index
 // ordering contract of the rasterizer relies on.
+#include "../../include/gs_b200.h"
 #include "gs_common.cuh"
 
 #include <algorithm>
@@ -422,6 +423,17 @@ int gs_sort_pairs_u32(uint32_t* keys, uint32_t* keys_alt, uint32_t* vals, uint32
     SortSegs sg; sg.n = 1; sg.off[0] = 0; sg.off[1] = n < 0 ? 0 : n;
     return gs_sort_pairs_segmented(keys, keys_alt, vals, vals_alt, sg, begin_bit, end_bit, scratch, result_in_alt,
                                    nullptr, 0, false, s);
+}
+
+extern "C" size_t gs_b200_sort_scratch_bytes(int64_t n) { return gs_sort_scratch_bytes(n); }
+
+extern "C" int32_t gs_b200_sort_pairs_u32(uint32_t* keys, uint32_t* keys_alt, uint32_t* vals, uint32_t* vals_alt, int64_t n,
+                                          int32_t begin_bit, int32_t end_bit, void* scratch, int32_t* result_in_alt,
+                                          void* stream) {
+    int r = 0;
+    int rc = gs_sort_pairs_u32(keys, keys_alt, vals, vals_alt, n, begin_bit, end_bit, scratch, &r, (cudaStream_t)stream);
+    if (result_in_alt) *result_in_alt = r;
+    return rc;
 }
 
 int gs_sort_pairs_segmented(uint32_t* keys, uint32_t* keys_alt, uint32_t* vals, uint32_t* vals_alt, const SortSegs& segs,

@@ -8,6 +8,7 @@
 //   densify_stats_kernel add_densification_stats + max_radii2D update (main_3DGS_renderer.py:767-769,
 //                        main_3DGS.py:210-213) fused.
 // All three are pure streaming kernels (HBM bound).
+#include "../../include/gs_b200.h"
 #include "gs_common.cuh"
 
 namespace {
@@ -131,8 +132,12 @@ densify_stats_kernel(int N, const float* __restrict__ g_means2D, const int32_t* 
 
 }  // namespace
 
-int gs_launch_activate(int N, const float* raw_opac, const float* raw_scales, const float* raw_rots, float* opac,
-                       float* scales, float* rots, cudaStream_t s) {
+extern "C" {
+
+int32_t gs_b200_activate(int32_t N, const float* raw_opac, const float* raw_scales, const float* raw_rots, float* opac,
+                         float* scales, float* rots, void* stream) {
+    if (N > 0 && (!raw_opac || !raw_scales || !raw_rots || !opac || !scales || !rots)) { gs_set_error("activate: NULL"); return 1; }
+    const cudaStream_t s = (cudaStream_t)stream;
     if (N <= 0) return 0;
     activate_kernel<<<(N + 255) / 256, 256, 0, s>>>(N, raw_opac, raw_scales, raw_rots, opac, scales, rots);
     gs_count_launches(1);
@@ -140,8 +145,11 @@ int gs_launch_activate(int N, const float* raw_opac, const float* raw_scales, co
     return 0;
 }
 
-int gs_launch_adam(int N, int M, const float* lrs6, double beta1, double beta2, float eps, int step, float grad_scale,
-                   const float* grads_packed, float* params_packed, float* m1, float* m2, cudaStream_t s) {
+int32_t gs_b200_adam_step(int32_t N, int32_t M, const float* lrs6, double beta1, double beta2, float eps, int32_t step,
+                          float grad_scale, const float* grads_packed, float* params_packed, float* m1, float* m2,
+                          void* stream) {
+    if (!lrs6 || step < 1 || (N > 0 && (!grads_packed || !params_packed || !m1 || !m2))) { gs_set_error("adam_step: bad argument"); return 1; }
+    const cudaStream_t s = (cudaStream_t)stream;
     if (N <= 0) return 0;
     AdamArgs a;
     const double bias1 = 1.0 - pow(beta1, (double)step);
@@ -171,11 +179,15 @@ int gs_launch_adam(int N, int M, const float* lrs6, double beta1, double beta2, 
     return 0;
 }
 
-int gs_launch_densify_stats(int N, const float* g_means2D, const int32_t* radii, float* grad_accum, float* denom,
-                            float* max_radii, cudaStream_t s) {
+int32_t gs_b200_densify_stats(int32_t N, const float* g_means2D, const int32_t* radii, float* grad_accum, float* denom,
+                              float* max_radii, void* stream) {
+    if (N > 0 && (!g_means2D || !radii || !grad_accum || !denom || !max_radii)) { gs_set_error("densify_stats: NULL"); return 1; }
+    const cudaStream_t s = (cudaStream_t)stream;
     if (N <= 0) return 0;
     densify_stats_kernel<<<(N + 255) / 256, 256, 0, s>>>(N, g_means2D, radii, grad_accum, denom, max_radii);
     gs_count_launches(1);
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
 }
+
+}  // extern "C"

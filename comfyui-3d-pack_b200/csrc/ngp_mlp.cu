@@ -8,6 +8,7 @@
 // dL/dx in the same pass, and reduces the weight gradients per CTA in shared memory (persistent CTAs, one set of
 // global atomics per CTA at the end).  fp32 SIMT on purpose: the reference runs these MLPs in fp32 and the cost is
 // ~3 kFMA/sample — far below the hash-grid gather/scatter around it, so tensor cores would not move the step time.
+#include "../../include/ngp_b200.h"
 #include "gs_common.cuh"
 
 namespace {
@@ -217,13 +218,19 @@ int launch_bwd(const float* X, long long N, const float* W1, const float* W2, co
 
 }  // namespace
 
-int ngp_mlp2_supported(int Din, int H, int Dout) {
+extern "C" {
+
+int32_t ngp_b200_mlp2_supported(int32_t Din, int32_t H, int32_t Dout) {
     return (H == 32 && (Din == 24 || Din == 32) && Dout >= 1 && Dout <= 4) ? 1 : 0;
 }
 
-int ngp_mlp2_fwd(const float* X, long long N, int Din, int H, int Dout, const float* W1, const float* W2, float* Y, cudaStream_t s) {
+int32_t ngp_b200_mlp2_fwd(const float* X, int64_t N, int32_t Din, int32_t H, int32_t Dout, const float* W1, const float* W2,
+                          float* Y, void* stream) {
+    GS_REQ(N == 0 || (X && W1 && W2 && Y), "NULL pointer");
+    GS_REQ(((size_t)X & 15) == 0, "X must be 16-byte aligned");
+    const cudaStream_t s = (cudaStream_t)stream;
     if (N <= 0) return 0;
-    if (!ngp_mlp2_supported(Din, H, Dout)) { gs_set_error("mlp2: unsupported dims %d-%d-%d", Din, H, Dout); return 1; }
+    if (!ngp_b200_mlp2_supported(Din, H, Dout)) { gs_set_error("mlp2: unsupported dims %d-%d-%d", Din, H, Dout); return 1; }
     int rc = 0;
     MLP_DISPATCH(launch_fwd, X, N, W1, W2, Y, s);
     if (rc) return rc;
@@ -232,10 +239,13 @@ int ngp_mlp2_fwd(const float* X, long long N, int Din, int H, int Dout, const fl
     return 0;
 }
 
-int ngp_mlp2_bwd(const float* X, long long N, int Din, int H, int Dout, const float* W1, const float* W2, const float* GY,
-                 float* GX, float* GW1, float* GW2, cudaStream_t s) {
+int32_t ngp_b200_mlp2_bwd(const float* X, int64_t N, int32_t Din, int32_t H, int32_t Dout, const float* W1, const float* W2,
+                          const float* GY, float* GX, float* GW1, float* GW2, void* stream) {
+    GS_REQ(N == 0 || (X && W1 && W2 && GY && GW1 && GW2), "NULL pointer");
+    GS_REQ(((size_t)X & 15) == 0 && ((size_t)GX & 15) == 0, "X/GX must be 16-byte aligned");
+    const cudaStream_t s = (cudaStream_t)stream;
     if (N <= 0) return 0;
-    if (!ngp_mlp2_supported(Din, H, Dout)) { gs_set_error("mlp2: unsupported dims %d-%d-%d", Din, H, Dout); return 1; }
+    if (!ngp_b200_mlp2_supported(Din, H, Dout)) { gs_set_error("mlp2: unsupported dims %d-%d-%d", Din, H, Dout); return 1; }
     int rc = 0;
     MLP_DISPATCH(launch_bwd, X, N, W1, W2, GY, GX, GW1, GW2, s);
     if (rc) return rc;
@@ -243,3 +253,5 @@ int ngp_mlp2_bwd(const float* X, long long N, int Din, int H, int Dout, const fl
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
 }
+
+}  // extern "C"

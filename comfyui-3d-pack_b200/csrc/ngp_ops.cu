@@ -7,6 +7,7 @@
 // weights / accumulate stream the packed samples once.
 // fp32 operation order of everything that decides an INTEGER output (corner indices, the packed sample list)
 // is pinned with __fmul_rn/__fadd_rn/__fdiv_rn to match oracle/ngp_oracle.py bit for bit.
+#include "../../include/ngp_b200.h"
 #include "gs_common.cuh"
 
 namespace {
@@ -347,8 +348,20 @@ int make_meta(GridMeta& gm, const int32_t* offsets_host, int L, float bound, dou
 
 #define NGP_GRID(n) (unsigned)(((n) + 255) / 256), 256
 
-int ngp_grid_encode_fwd(const float* x, long long N, const float* emb, const int32_t* offsets_host, int L, float bound,
-                        double pls, int base, float* out, cudaStream_t s) {
+static MarchArgs make_march(const float* aabb, float near_plane, float far_plane, float dt, int R) {
+    MarchArgs ma;
+    for (int a = 0; a < 3; a++) { ma.lo[a] = aabb[a]; ma.hi[a] = aabb[3 + a]; }
+    ma.near_plane = near_plane; ma.far_plane = far_plane; ma.dt = dt; ma.R = R;
+    return ma;
+}
+
+extern "C" {
+
+int32_t ngp_b200_grid_encode_fwd(const float* x, int64_t N, const float* emb, const int32_t* offsets_host, int32_t L,
+                                 float bound, double pls, int32_t base, float* out, void* stream) {
+    GS_REQ(N == 0 || (x && emb && offsets_host && out), "NULL pointer");
+    GS_REQ(((size_t)emb & 7) == 0 && ((size_t)out & 7) == 0, "emb/out must be 8-byte aligned");
+    const cudaStream_t s = (cudaStream_t)stream;
     if (N <= 0) return 0;
     GridMeta gm; if (make_meta(gm, offsets_host, L, bound, pls, base)) return 1;
     grid_encode_fwd_kernel<<<NGP_GRID(N * L), 0, s>>>(x, N, (const float2*)emb, gm, (float2*)out);
@@ -356,8 +369,10 @@ int ngp_grid_encode_fwd(const float* x, long long N, const float* emb, const int
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
 }
-int ngp_grid_encode_bwd(const float* x, long long N, const int32_t* offsets_host, int L, float bound, double pls, int base,
-                        const float* g_out, float* d_emb, cudaStream_t s) {
+int32_t ngp_b200_grid_encode_bwd(const float* x, int64_t N, const int32_t* offsets_host, int32_t L, float bound, double pls,
+                                 int32_t base, const float* g_out, float* d_emb, void* stream) {
+    GS_REQ(N == 0 || (x && offsets_host && g_out && d_emb), "NULL pointer");
+    const cudaStream_t s = (cudaStream_t)stream;
     if (N <= 0) return 0;
     GridMeta gm; if (make_meta(gm, offsets_host, L, bound, pls, base)) return 1;
     const bool v4 = ((uintptr_t)d_emb & 15) == 0;
@@ -378,8 +393,10 @@ int ngp_grid_encode_bwd(const float* x, long long N, const int32_t* offsets_host
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
 }
-int ngp_grid_tv(const float* x, long long N, const float* emb, const int32_t* offsets_host, int L, float bound, double pls,
-                int base, float weight, float* d_emb, cudaStream_t s) {
+int32_t ngp_b200_grid_tv_grad(const float* x, int64_t N, const float* emb, const int32_t* offsets_host, int32_t L,
+                              float bound, double pls, int32_t base, float weight, float* d_emb, void* stream) {
+    GS_REQ(N == 0 || (x && emb && offsets_host && d_emb), "NULL pointer");
+    const cudaStream_t s = (cudaStream_t)stream;
     if (N <= 0) return 0;
     GridMeta gm; if (make_meta(gm, offsets_host, L, bound, pls, base)) return 1;
     grid_tv_kernel<<<NGP_GRID(N * L), 0, s>>>(x, N, (const float2*)emb, gm, weight, (float2*)d_emb);
@@ -388,20 +405,17 @@ int ngp_grid_tv(const float* x, long long N, const float* emb, const int32_t* of
     return 0;
 }
 
-size_t ngp_march_scratch_bytes(long long n_rays, int R) {
+size_t ngp_b200_march_scratch_bytes(int64_t n_rays, int32_t R) {
     return (((size_t)R * R * R + 31) / 32) * 4 + 256 + gs_scan_scratch_bytes(n_rays);
 }
 
-static MarchArgs make_march(const float* aabb, float near_plane, float far_plane, float dt, int R) {
-    MarchArgs ma;
-    for (int a = 0; a < 3; a++) { ma.lo[a] = aabb[a]; ma.hi[a] = aabb[3 + a]; }
-    ma.near_plane = near_plane; ma.far_plane = far_plane; ma.dt = dt; ma.R = R;
-    return ma;
-}
-
-int ngp_march_count(const float* rays_o, const float* rays_d, long long n_rays, const uint8_t* binary, int R,
-                    const float* aabb, float near_plane, float far_plane, float dt, const float* t_offset, uint32_t* counts,
-                    uint32_t* offsets, unsigned long long* total_dev, void* scratch, cudaStream_t s) {
+int32_t ngp_b200_march_count(const float* rays_o, const float* rays_d, int64_t n_rays, const uint8_t* binary, int32_t R,
+                             const float* aabb, float near_plane, float far_plane, float dt, const float* t_offset,
+                             uint32_t* counts, uint32_t* offsets, unsigned long long* total_dev, void* scratch,
+                             void* stream) {
+    GS_REQ(binary && aabb && counts && offsets && total_dev && scratch && (n_rays == 0 || (rays_o && rays_d)), "NULL pointer");
+    GS_REQ(dt > 0.f && R > 0, "bad step / resolution");
+    const cudaStream_t s = (cudaStream_t)stream;
     const int ncell = R * R * R, nwords = (ncell + 31) / 32;
     if ((size_t)nwords * 4 > 200 * 1024) { gs_set_error("march: occupancy grid %d^3 does not fit shared memory", R); return 1; }
     uint32_t* bits = (uint32_t*)scratch;
@@ -419,47 +433,60 @@ int ngp_march_count(const float* rays_o, const float* rays_d, long long n_rays, 
     return 0;
 }
 
-int ngp_march_write(const float* rays_o, const float* rays_d, long long n_rays, int R, const float* aabb, float near_plane,
-                    float far_plane, float dt, const float* t_offset, const uint32_t* offsets, long long* ray_indices,
-                    float* t_starts, float* t_ends, void* scratch, cudaStream_t s) {
+int32_t ngp_b200_march_write(const float* rays_o, const float* rays_d, int64_t n_rays, int32_t R, const float* aabb,
+                             float near_plane, float far_plane, float dt, const float* t_offset, const uint32_t* offsets,
+                             int64_t* ray_indices, float* t_starts, float* t_ends, void* scratch, void* stream) {
+    GS_REQ(aabb && offsets && scratch && (n_rays == 0 || (rays_o && rays_d)), "NULL pointer");
+    const cudaStream_t s = (cudaStream_t)stream;
     if (n_rays <= 0) return 0;
     const int nwords = (R * R * R + 31) / 32;
     const size_t smem = (size_t)nwords * 4;
     if (smem > 48 * 1024) GS_CUDA_CHECK(cudaFuncSetAttribute(march_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     march_kernel<true><<<NGP_GRID(n_rays), smem, s>>>(rays_o, rays_d, n_rays, (const uint32_t*)scratch,
                                                       make_march(aabb, near_plane, far_plane, dt, R), t_offset, nullptr, offsets,
-                                                      ray_indices, t_starts, t_ends);
+                                                      (long long*)ray_indices, t_starts, t_ends);
     gs_count_launches(1);
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
 }
 
-int ngp_ray_ranges(const long long* ri, long long S, long long n_rays, int32_t* ranges, cudaStream_t s) {
+int32_t ngp_b200_ray_ranges(const int64_t* ri, int64_t S, int64_t n_rays, int32_t* ranges, void* stream) {
+    GS_REQ(ranges && (S == 0 || ri), "NULL pointer");
+    const cudaStream_t s = (cudaStream_t)stream;
     GS_CUDA_CHECK(cudaMemsetAsync(ranges, 0, (size_t)n_rays * 8, s));
     if (S <= 0) return 0;
-    ray_ranges_kernel<<<NGP_GRID(S), 0, s>>>(ri, S, ranges);
-    ray_counts_kernel<<<NGP_GRID(S), 0, s>>>(ri, S, ranges);
+    ray_ranges_kernel<<<NGP_GRID(S), 0, s>>>((const long long*)ri, S, ranges);
+    ray_counts_kernel<<<NGP_GRID(S), 0, s>>>((const long long*)ri, S, ranges);
     gs_count_launches(2);
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
 }
-int ngp_weights_fwd(const float* ts, const float* te, const float* sig, const int32_t* ranges, long long n_rays, float* w,
-                    float* tr, float* al, cudaStream_t s) {
+int32_t ngp_b200_weights_fwd(const float* ts, const float* te, const float* sig, const int32_t* ranges, int64_t n_rays,
+                             float* w, float* tr, float* al, void* stream) {
+    GS_REQ(ranges, "NULL ranges");
+    const cudaStream_t s = (cudaStream_t)stream;
     if (n_rays <= 0) return 0;
     weights_fwd_kernel<<<(unsigned)((n_rays + 127) / 128), 128, 0, s>>>(ts, te, sig, ranges, n_rays, w, tr, al);
     gs_count_launches(1);
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
 }
-int ngp_weights_bwd(const float* ts, const float* te, const int32_t* ranges, long long n_rays, const float* tr, const float* al,
-                    const float* gw, const float* gt, const float* ga, float* dsig, cudaStream_t s) {
+int32_t ngp_b200_weights_bwd(const float* ts, const float* te, const float* sig, const int32_t* ranges, int64_t n_rays,
+                             const float* tr, const float* al, const float* gw, const float* gt, const float* ga, float* dsig,
+                             void* stream) {
+    (void)sig;
+    GS_REQ(ranges, "NULL ranges");
+    const cudaStream_t s = (cudaStream_t)stream;
     if (n_rays <= 0) return 0;
     weights_bwd_kernel<<<(unsigned)((n_rays + 127) / 128), 128, 0, s>>>(ts, te, ranges, n_rays, tr, al, gw, gt, ga, dsig);
     gs_count_launches(1);
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
 }
-int ngp_accumulate_fwd(const float* w, const float* v, int C, const int32_t* ranges, long long n_rays, float* out, cudaStream_t s) {
+int32_t ngp_b200_accumulate_fwd(const float* w, const float* v, int32_t C, const int32_t* ranges, int64_t n_rays, float* out,
+                                void* stream) {
+    GS_REQ(ranges && out, "NULL pointer");
+    const cudaStream_t s = (cudaStream_t)stream;
     if (n_rays <= 0) return 0;
     if (C < 1 || C > 4) { gs_set_error("accumulate: 1..4 channels supported, got %d", C); return 1; }
     accumulate_fwd_kernel<<<(unsigned)((n_rays + 127) / 128), 128, 0, s>>>(w, v, C, ranges, n_rays, out);
@@ -467,11 +494,15 @@ int ngp_accumulate_fwd(const float* w, const float* v, int C, const int32_t* ran
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
 }
-int ngp_accumulate_bwd(const float* w, const float* v, int C, const long long* ri, long long S, const float* g_out, float* dw,
-                       float* dv, cudaStream_t s) {
+int32_t ngp_b200_accumulate_bwd(const float* w, const float* v, int32_t C, const int64_t* ri, int64_t S, const float* g_out,
+                                float* dw, float* dv, void* stream) {
+    GS_REQ(S == 0 || (w && ri && g_out && dw), "NULL pointer");
+    const cudaStream_t s = (cudaStream_t)stream;
     if (S <= 0) return 0;
-    accumulate_bwd_kernel<<<NGP_GRID(S), 0, s>>>(w, v, C, ri, S, g_out, dw, dv);
+    accumulate_bwd_kernel<<<NGP_GRID(S), 0, s>>>(w, v, C, (const long long*)ri, S, g_out, dw, dv);
     gs_count_launches(1);
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
 }
+
+}  // extern "C"

@@ -9,7 +9,7 @@
 // is the 64-bit key (z bits << 32) | packed index; z > 0, so the keys order as (z, index) and every pixel's selection is
 // a minimum over a set, independent of the order the atomics land in.  Slot k of a pixel is filled by pass k, a 64-bit
 // atomicMin over the candidates strictly greater than slot k - 1, so K passes give the K smallest keys, sorted.
-#include "gs_b200_pts.h"
+#include "../../include/gs_b200_pts.h"
 #include "gs_common.cuh"
 
 #include <math.h>

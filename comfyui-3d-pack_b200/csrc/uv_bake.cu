@@ -42,6 +42,7 @@
 // angle at a below ~0.45 degrees), denom < 0, d00 or d11 outside [2^-60, 2^60], or a non-finite bound.  A face with
 // denom == 0 or NaN, or a non-finite UV (which makes denom NaN), can never hit (v or w is then NaN or +-inf, or
 // v + w = +inf) and is dropped.
+#include "../../include/dr_b200.h"
 #include "gs_common.cuh"
 
 namespace {
@@ -242,10 +243,20 @@ ub_interp_kernel(const float* __restrict__ attr, int NV, const int32_t* __restri
 
 }  // namespace
 
-size_t ub_scratch_bytes(int F, int res) { return 256 + (size_t)res * res * 4 + (size_t)F * 8; }
+extern "C" {
 
-int ub_launch_rasterize(const float* uv, int NV, const int32_t* T, int NF, float* out, int res, int rows, int cols,
-                        void* scratch, cudaStream_t s) {
+size_t dr_b200_uvbake_scratch_bytes(int32_t F, int32_t res) {
+    return (F < 0 || res <= 0 || res > (1 << 15)) ? 0 : 256 + (size_t)res * res * 4 + (size_t)F * 8;
+}
+
+int32_t dr_b200_uvbake_rasterize(const float* uv, int32_t NV, const int32_t* T, int32_t NF, float* out, int32_t res,
+                                 int32_t rows, int32_t cols, void* scratch, void* stream) {
+    GS_REQ(NV >= 0 && NF >= 0 && res > 0 && res <= (1 << 15) && rows >= 0 && cols >= 0, "bad sizes");
+    GS_REQ(out && scratch && (NF == 0 || (uv && T)), "NULL pointer");
+    GS_REQ(((size_t)uv & 7) == 0 && ((size_t)out & 15) == 0, "uv must be 8-byte and out 16-byte aligned");
+    const cudaStream_t s = (cudaStream_t)stream;
+    rows = rows < res ? rows : res;
+    cols = cols < res ? cols : res;
     if (rows <= 0 || cols <= 0) return 0;
     const size_t n = (size_t)rows * cols;
     uint32_t* counts = (uint32_t*)scratch;
@@ -266,8 +277,14 @@ int ub_launch_rasterize(const float* uv, int NV, const int32_t* T, int NF, float
     return 0;
 }
 
-int ub_launch_interpolate(const float* attr, int NV, const int32_t* T, int NF, const float* rast, float* out, int res,
-                          int rows, int cols, cudaStream_t s) {
+int32_t dr_b200_uvbake_interpolate(const float* attr, int32_t NV, const int32_t* T, int32_t NF, const float* rast,
+                                   float* out, int32_t res, int32_t rows, int32_t cols, void* stream) {
+    GS_REQ(NV >= 0 && NF >= 0 && res > 0 && res <= (1 << 15) && rows >= 0 && cols >= 0, "bad sizes");
+    GS_REQ(rast && out && (NF == 0 || T) && (NV == 0 || attr), "NULL pointer");
+    GS_REQ(((size_t)rast & 15) == 0, "rast must be 16-byte aligned");
+    const cudaStream_t s = (cudaStream_t)stream;
+    rows = rows < res ? rows : res;
+    cols = cols < res ? cols : res;
     if (rows <= 0 || cols <= 0) return 0;
     const size_t n = (size_t)rows * cols;
     ub_interp_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(attr, NV, T, NF, (const float4*)rast, res, rows, cols, out);
@@ -275,3 +292,5 @@ int ub_launch_interpolate(const float* attr, int NV, const int32_t* T, int NF, c
     GS_CUDA_CHECK(cudaGetLastError());
     return 0;
 }
+
+}  // extern "C"

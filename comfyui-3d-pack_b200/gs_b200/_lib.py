@@ -1,4 +1,4 @@
-"""ctypes binding of the C ABI declared in include/{gs,dr,ngp}_b200.h.
+"""ctypes binding of the C ABI declared in include/*.h.
 
 Every function the headers declare is bound at import with the restype / argtypes its prototype gives, and every
 integer `#define GS_B200_<NAME>` and `enum { GS_B200_<NAME> = n }` becomes the module attribute `<NAME>`, so the
@@ -17,7 +17,6 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libgs_b200.so")
 _INCLUDE = os.path.join(os.path.dirname(os.path.dirname(_HERE)), "include")
-_HEADERS = ("gs_b200.h", "dr_b200.h", "ngp_b200.h")
 
 
 class View(C.Structure):
@@ -87,37 +86,19 @@ if not os.path.exists(LIB_PATH):
 lib = C.CDLL(LIB_PATH)
 
 
-def _bind_header(handle, h):
-    """Bind every function header `h` (a name under include/, or a path) declares on `handle`; returns the header's
-    constants."""
-    path = os.path.join(_INCLUDE, h)
-    if not os.path.exists(path):
-        raise ImportError(f"{path} is missing: gs_b200 binds its libraries from the headers under include/.")
-    with open(path) as f:
-        src = f.read()
-    for name, (restype, argtypes) in prototypes(src).items():
-        fn = getattr(handle, name)
-        fn.restype, fn.argtypes = restype, argtypes
-    return constants(src)
-
-
 def _bind():
-    for h in _HEADERS:
-        globals().update(_bind_header(lib, h))
+    if not os.path.isdir(_INCLUDE):
+        raise ImportError(f"{_INCLUDE} is missing: gs_b200 binds its library from the headers there.")
+    for h in sorted(f for f in os.listdir(_INCLUDE) if f.endswith(".h")):
+        with open(os.path.join(_INCLUDE, h)) as f:
+            src = f.read()
+        for name, (restype, argtypes) in prototypes(src).items():
+            fn = getattr(lib, name)
+            fn.restype, fn.argtypes = restype, argtypes
+        globals().update(constants(src))
 
 
 _bind()
-
-
-def companion(so_name, header):
-    """(handle, constants) of a library built beside libgs_b200.so and linked against it (csrc/build.sh), bound from
-    its own header (a path) in the same way.  Raises ImportError when it has not been built."""
-    path = os.path.join(_HERE, so_name)
-    if not os.path.exists(path):
-        raise ImportError(f"{path} is missing: the sm_90a CUDA library has not been built. "
-                          "Run `python __graft_entry__.py` (or comfyui-3d-pack_b200/csrc/build.sh). There is no CPU fallback.")
-    handle = C.CDLL(path)
-    return handle, _bind_header(handle, header)
 
 
 def last_error() -> str:

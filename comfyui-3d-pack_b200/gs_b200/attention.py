@@ -1,5 +1,5 @@
-"""Multi-head attention forward on the GPU: the sm_90a kernel behind gs_b200_attn_forward (libgs_attn.so, declared in
-csrc/gs_b200_attn.h, which states every rule), as the two calls the `flash_attn` import name
+"""Multi-head attention forward on the GPU: the sm_90a kernel behind gs_b200_attn_forward (declared in
+include/gs_b200_attn.h, which states every rule), as the two calls the `flash_attn` import name
 (comfyui-3d-pack_b200/flash_attn) builds on.
 
 - varlen(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k): q [total_q, H, 64], k / v [total_k, H, 64];
@@ -16,17 +16,14 @@ csrc/gs_b200_attn.h, which states every rule), as the two calls the `flash_attn`
 - Work goes on the current stream; cu_seqlens is never read back to the host.
 """
 import ctypes as C
-import os
 
 import torch
 
 from . import _lib
-from ._lib import ptr, stream
+from ._lib import lib, ptr, stream
 
-HEADER = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "csrc", "gs_b200_attn.h")
-lib, CONSTANTS = _lib.companion("libgs_attn.so", HEADER)
-HEAD_DIM = CONSTANTS["ATTN_HEAD_DIM"]
-_DTYPES = {torch.float16: CONSTANTS["ATTN_F16"], torch.bfloat16: CONSTANTS["ATTN_BF16"]}
+HEAD_DIM = _lib.ATTN_HEAD_DIM
+_DTYPES = {torch.float16: _lib.ATTN_F16, torch.bfloat16: _lib.ATTN_BF16}
 
 
 def _tensor(name, arg, t):

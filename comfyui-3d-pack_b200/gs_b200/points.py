@@ -1,5 +1,5 @@
 """pytorch3d's point rasterizer and TriplaneGaussian's points_projection on the GPU: the sm_90a kernels behind
-gs_b200_pts_* (libgs_pts.so, bound from csrc/gs_b200_pts.h, which states every rule), under the names TriplaneGaussian
+gs_b200_pts_* (declared in include/gs_b200_pts.h, which states every rule), under the names TriplaneGaussian
 imports from pytorch3d (`utils/ops.py`, `models/snowflake/model_spdpp.py`).  This is a module, not a `pytorch3d`
 package: callers take it in by changing their import lines.
 
@@ -23,17 +23,14 @@ package: callers take it in by changing their import lines.
 
 import ctypes as C
 import dataclasses
-import os
 from typing import NamedTuple, Optional, Sequence, Union
 
 import torch
 
 from . import _lib
-from ._lib import ptr, stream
+from ._lib import lib, ptr, stream
 
-HEADER = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "csrc", "gs_b200_pts.h")
-lib, CONSTANTS = _lib.companion("libgs_pts.so", HEADER)
-MAX_K = CONSTANTS["PTS_MAX_K"]
+MAX_K = _lib.PTS_MAX_K
 
 
 class PointFragments(NamedTuple):

@@ -1,5 +1,5 @@
 """numpy oracle of the point rasterizer and points_projection (gs_b200.points; rules in
-comfyui-3d-pack_b200/csrc/gs_b200_pts.h), written from those rules with no pytorch3d.
+include/gs_b200_pts.h), written from those rules with no pytorch3d.
 
 - Projection, pixel centres and squared distances are defined in fp32, one rounding per operation, so they are
   restated here in numpy float32 in the header's operation order (numpy rounds every float32 operation and never

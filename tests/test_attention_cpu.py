@@ -249,21 +249,18 @@ def test_argument_errors_before_gpu_work():
 
 
 # ---- ABI ------------------------------------------------------------------------------------------------------------
-def test_abi_symbol_and_constants():
-    """gs_b200_attn_forward lives in libgs_attn.so, bound from csrc/gs_b200_attn.h; its argument errors are
-    reported through libgs_b200's gs_b200_last_error, and the core library's headers do not declare it"""
+def test_abi_is_bound_from_include_with_its_constants():
+    """gs_b200_attn_forward is bound from include/gs_b200_attn.h, with its constants; its argument errors are reported
+    through gs_b200_last_error"""
     import ctypes as C
-    from gs_b200 import _lib, attention as A
-    assert {k: A.CONSTANTS[k] for k in ("ATTN_F16", "ATTN_BF16", "ATTN_HEAD_DIM")} == \
-        {"ATTN_F16": 0, "ATTN_BF16": 1, "ATTN_HEAD_DIM": 64}
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    protos = _lib.prototypes(open(A.HEADER).read())
+    from gs_b200 import _lib
+    assert (_lib.ATTN_F16, _lib.ATTN_BF16, _lib.ATTN_HEAD_DIM) == (0, 1, 64)
+    header = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "include", "gs_b200_attn.h")
+    protos = _lib.prototypes(open(header).read())
     assert list(protos) == ["gs_b200_attn_forward"]
-    for h in _lib._HEADERS:
-        assert "gs_b200_attn_forward" not in _lib.prototypes(open(os.path.join(root, "include", h)).read())
     import subprocess
-    subprocess.run(["gcc", "-std=c99", "-Wall", "-Werror", "-fsyntax-only", "-x", "c", A.HEADER], check=True)
-    fn = A.lib.gs_b200_attn_forward
+    subprocess.run(["gcc", "-std=c99", "-Wall", "-Werror", "-fsyntax-only", "-x", "c", header], check=True)
+    fn = _lib.lib.gs_b200_attn_forward
     assert fn.restype is C.c_int32 and len(fn.argtypes) == 22
     assert fn.argtypes[19] is C.c_float
     # invalid arguments are refused before any launch, with a message

@@ -38,13 +38,13 @@ def test_library_exports_every_declared_symbol():
     assert lib.gs_b200_abi_version() == 1
 
 
-def test_every_header_is_plain_c_and_every_declared_entry_point_is_exported():
-    """include/*.h (gs, dr, ngp): each compiles as C on its own (no C++ / torch types in the boundary) and every
-    function it declares is an exported symbol of libgs_b200.so."""
+def test_all_five_headers_are_plain_c_and_every_declared_entry_point_is_exported():
+    """include/*.h (gs, dr, ngp, attention, points): each compiles as C on its own (no C++ / torch types in the
+    boundary) and every function it declares is an exported symbol of libgs_b200.so."""
     lib = ctypes.CDLL(_ensure_built())
     inc = os.path.join(ROOT, "include")
     headers = sorted(f for f in os.listdir(inc) if f.endswith(".h"))
-    assert headers == ["dr_b200.h", "gs_b200.h", "ngp_b200.h"]
+    assert headers == ["dr_b200.h", "gs_b200.h", "gs_b200_attn.h", "gs_b200_pts.h", "ngp_b200.h"]
     total = 0
     for h in headers:
         subprocess.run(["gcc", "-std=c99", "-Wall", "-Werror", "-fsyntax-only", "-x", "c", os.path.join(inc, h)], check=True)
@@ -78,18 +78,18 @@ def test_ctypes_structs_match_header_layout():
     assert ctypes.sizeof(_lib.State) == ss and _lib.State.num_rendered.offset == onr and _lib.State.owned.offset == oo
 
 
-def test_ctypes_binding_is_derived_from_the_headers():
+def test_ctypes_binding_is_derived_from_every_header_in_include():
     """gs_b200._lib binds every function include/*.h declares, with one argtype per declared parameter; a few
     signatures are pinned by hand (every row of the C -> ctypes mapping), the header constants reach Python, and a
     by-value type the mapping does not know is refused rather than guessed."""
     from gs_b200 import _lib
     declared = {}
-    for h in ("gs_b200.h", "dr_b200.h", "ngp_b200.h"):
+    for h in sorted(f for f in os.listdir(os.path.join(ROOT, "include")) if f.endswith(".h")):
         src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", h)).read(), flags=re.S)
         for name, params in re.findall(r"\b((?:gs|dr|ngp)_b200_\w+)\s*\(([^()]*)\)\s*;", src):
             declared[name] = 0 if params.strip() == "void" else params.count(",") + 1
     bound = {n for n, f in vars(_lib.lib).items() if isinstance(f, _lib.lib._FuncPtr)}
-    assert len(declared) == 100 and bound == set(declared)
+    assert len(declared) == 105 and bound == set(declared)
     for name, nparams in declared.items():
         assert len(getattr(_lib.lib, name).argtypes) == nparams, name
 
@@ -105,6 +105,8 @@ def test_ctypes_binding_is_derived_from_the_headers():
                                       (_lib.ALLOC_FN, P, ctypes.POINTER(_lib.State), P)),
         "gs_b200_step_device_hook": (I, (I, I, I, I, F, P, P, I, I) + (P,) * 9 + (_lib.VIEW_HOOK, P, P, P)),
         "gs_b200_set_grad_sink": (I, (_lib.GRAD_SINK, P, I)),
+        "gs_b200_attn_forward": (I, (I, I, I, I) + (P, L, L) * 3 + (P, P, L, L, L, L, F, P, P)),
+        "gs_b200_pts_rasterize": (I, (I, L, I, I, I, F, I) + (P,) * 11),
     }
     for name, (restype, argtypes) in expected.items():
         fn = getattr(_lib.lib, name)
@@ -117,6 +119,52 @@ def test_ctypes_binding_is_derived_from_the_headers():
     assert _lib.prototypes("int32_t gs_b200_x(const uint8_t* x, void* stream);") == {"gs_b200_x": (I, [P, P])}
     with pytest.raises(ImportError, match="gs_b200_x.*uint8_t"):
         _lib.prototypes("int32_t gs_b200_x(uint8_t x);")
+
+
+def test_dr_and_ngp_entry_points_refuse_bad_arguments_with_their_messages():
+    """Every dr_b200_* / ngp_b200_* entry point, called with arguments that fail its first check, returns 1 and sets
+    gs_b200_last_error() to exactly "<entry point>: <message>", with no GPU work.  The size and capability queries,
+    which have no error path, return their documented values (0 for invalid arguments)."""
+    from gs_b200 import _lib
+    lib, N = _lib.lib, None
+    refused = {
+        "dr_b200_rasterize_fwd": ((N, N, -1, 0, 0, 1, 1, N, N, N, N), "bad sizes"),
+        "dr_b200_rasterize_bwd": ((N, N, 1, 1, 1, 1, 1, N, N, N, N), "NULL pointer"),
+        "dr_b200_interpolate_fwd": ((N, 1, N, N, N, 1, 1, 1, 1, 1, 1, N, N, N), "NULL pointer"),
+        "dr_b200_interpolate_bwd": ((N, 1, N, N, N, 1, 1, 1, 1, 1, 1, N, N, N, N, N, N), "NULL pointer"),
+        "dr_b200_texture_fwd": ((N, 1, 1, 1, 1, N, 1, 1, 1, 0, N, N), "bad argument"),
+        "dr_b200_texture_bwd": ((N, 1, 1, 1, 1, N, 1, 1, 1, 0, N, N, N, N), "NULL pointer"),
+        "dr_b200_edge_opposites": ((N, 1, 3, N, N, N), "NULL pointer"),
+        "dr_b200_antialias_fwd": ((N, N, N, N, N, 1, 1, 1, 1, 1, 1, N, N), "NULL pointer"),
+        "dr_b200_antialias_bwd": ((N, N, N, N, N, 1, 1, 1, 1, 1, 1, N, N, N, N), "NULL pointer"),
+        "dr_b200_cr_rasterize": ((N, -1, N, 0, N, 1, 1, 0.0, N, N, N, N), "bad sizes"),
+        "dr_b200_cr_interpolate_fwd": ((N, -1, 1, N, 0, N, N, 0, 0, 0, N, N), "bad sizes"),
+        "dr_b200_cr_interpolate_bwd": ((N, -1, 1, N, 0, N, N, 0, 0, 0, N, N, N, N, N), "bad sizes"),
+        "dr_b200_uvbake_rasterize": ((N, 0, N, 0, N, 0, 0, 0, N, N), "bad sizes"),
+        "dr_b200_uvbake_interpolate": ((N, 0, N, 0, N, N, 0, 0, 0, N), "bad sizes"),
+        "ngp_b200_grid_encode_fwd": ((N, 1, N, N, 1, 1.0, 2.0, 16, N, N), "NULL pointer"),
+        "ngp_b200_grid_encode_bwd": ((N, 1, N, 1, 1.0, 2.0, 16, N, N, N), "NULL pointer"),
+        "ngp_b200_grid_tv_grad": ((N, 1, N, N, 1, 1.0, 2.0, 16, 1.0, N, N), "NULL pointer"),
+        "ngp_b200_march_count": ((N, N, 1, N, 1, N, 0.0, 1.0, 0.1, N, N, N, N, N, N), "NULL pointer"),
+        "ngp_b200_march_write": ((N, N, 1, 1, N, 0.0, 1.0, 0.1, N, N, N, N, N, N, N), "NULL pointer"),
+        "ngp_b200_ray_ranges": ((N, 1, 1, N, N), "NULL pointer"),
+        "ngp_b200_weights_fwd": ((N, N, N, N, 1, N, N, N, N), "NULL ranges"),
+        "ngp_b200_weights_bwd": ((N, N, N, N, 1, N, N, N, N, N, N, N), "NULL ranges"),
+        "ngp_b200_accumulate_fwd": ((N, N, 1, N, 1, N, N), "NULL pointer"),
+        "ngp_b200_accumulate_bwd": ((N, N, 1, N, 1, N, N, N, N), "NULL pointer"),
+        "ngp_b200_mlp2_fwd": ((N, 1, 24, 32, 1, N, N, N, N), "NULL pointer"),
+        "ngp_b200_mlp2_bwd": ((N, 1, 24, 32, 1, N, N, N, N, N, N, N), "NULL pointer"),
+    }
+    for name, (args, msg) in refused.items():
+        assert getattr(lib, name)(*args) == 1, name
+        assert _lib.last_error() == f"{name}: {msg}"
+
+    assert lib.dr_b200_rasterize_scratch_bytes(1, 1, 1, 1) == 8 + 256 + (2 + 4096) * 8 + 4
+    assert lib.dr_b200_topology_scratch_bytes(1) == 4 * 256 + lib.gs_b200_sort_scratch_bytes(3) + 256
+    assert lib.dr_b200_cr_scratch_bytes(-1, 1, 1) == 0 and lib.dr_b200_cr_scratch_bytes(1, 2, 2) == 2 * 2 * 8 + 256 + 8
+    assert lib.dr_b200_uvbake_scratch_bytes(1, 1 << 16) == 0 and lib.dr_b200_uvbake_scratch_bytes(1, 2) == 256 + 16 + 8
+    assert lib.ngp_b200_march_scratch_bytes(1, 64) - lib.ngp_b200_march_scratch_bytes(1, 32) == (64 ** 3 - 32 ** 3) // 8
+    assert lib.ngp_b200_mlp2_supported(24, 32, 1) == 1 and lib.ngp_b200_mlp2_supported(16, 32, 1) == 0
 
 
 def test_settings_namedtuple_field_order_matches_reference_call_site():

@@ -195,25 +195,23 @@ def test_settings_and_argument_errors_before_any_gpu_work():
     assert (s.image_size, s.radius, s.points_per_pixel, s.bin_size, s.max_points_per_bin) == ((252, 180), 0.0075, 1, 0, None)
 
 
-def test_c_abi_is_bound_from_its_header():
-    """gs_b200_pts_* live in libgs_pts.so and are bound from csrc/gs_b200_pts.h: every declared function resolves with
-    one argtype per parameter, and libgs_b200.so's own headers declare none of them."""
+def test_c_abi_is_bound_from_include():
+    """gs_b200_pts_* are bound from include/gs_b200_pts.h: every declared function resolves with one argtype per
+    parameter."""
     from gs_b200 import _lib
     from gs_b200 import points as P
-    src = re.sub(r"/\*.*?\*/", "", open(P.HEADER).read(), flags=re.S)
+    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "gs_b200_pts.h")).read(), flags=re.S)
     declared = dict(re.findall(r"\b(gs_b200_pts_\w+)\s*\(([^()]*)\)\s*;", src))
     assert set(declared) == {"gs_b200_pts_scratch_bytes", "gs_b200_pts_rasterize", "gs_b200_pts_lift",
                              "gs_b200_pts_lift_backward"}
     for name, params in declared.items():
-        assert len(getattr(P.lib, name).argtypes) == params.count(",") + 1, name
+        assert len(getattr(_lib.lib, name).argtypes) == params.count(",") + 1, name
     I, L, F, V = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_void_p
-    assert (P.lib.gs_b200_pts_rasterize.restype, tuple(P.lib.gs_b200_pts_rasterize.argtypes)) == \
+    assert (_lib.lib.gs_b200_pts_rasterize.restype, tuple(_lib.lib.gs_b200_pts_rasterize.argtypes)) == \
         (I, (I, L, I, I, I, F, I) + (V,) * 11)
-    assert P.lib.gs_b200_pts_scratch_bytes.restype == ctypes.c_size_t and P.MAX_K == 8
-    for h in ("gs_b200.h", "dr_b200.h", "ngp_b200.h"):
-        assert "gs_b200_pts_" not in open(os.path.join(ROOT, "include", h)).read()
-    # argument errors come back through libgs_b200's error string, with no GPU work
-    assert P.lib.gs_b200_pts_scratch_bytes(1, 10, 4, 4, 9) == 0 and "K 9" in _lib.last_error()
-    assert P.lib.gs_b200_pts_scratch_bytes(0, 10, 4, 4, 1) == 0
-    assert P.lib.gs_b200_pts_scratch_bytes(2, 10, 4, 4, 3) >= 2 * 16 * 3 * 8 + 10 * 16
-    assert P.lib.gs_b200_pts_rasterize(1, 4, 4, 4, 1, -1.0, 1, *([None] * 11)) == 1 and "radius" in _lib.last_error()
+    assert _lib.lib.gs_b200_pts_scratch_bytes.restype == ctypes.c_size_t and P.MAX_K == 8
+    # argument errors come back through gs_b200_last_error, with no GPU work
+    assert _lib.lib.gs_b200_pts_scratch_bytes(1, 10, 4, 4, 9) == 0 and "K 9" in _lib.last_error()
+    assert _lib.lib.gs_b200_pts_scratch_bytes(0, 10, 4, 4, 1) == 0
+    assert _lib.lib.gs_b200_pts_scratch_bytes(2, 10, 4, 4, 3) >= 2 * 16 * 3 * 8 + 10 * 16
+    assert _lib.lib.gs_b200_pts_rasterize(1, 4, 4, 4, 1, -1.0, 1, *([None] * 11)) == 1 and "radius" in _lib.last_error()
