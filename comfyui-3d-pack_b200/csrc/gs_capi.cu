@@ -1103,6 +1103,43 @@ int32_t gs_b200_debug_bin_views(int32_t V, int32_t H, int32_t W, int32_t sh_degr
     return 0;
 }
 
+// The multi-view step's batched preprocess, as step_core runs it (StepChunks, chunk_ws_setup, chunk_bin_a; with
+// geom_only the host-buffer step's colour-free pass, then gs_launch_sh_colour_multi), with the records copied out.
+int32_t gs_b200_debug_preprocess_views(int32_t V, int32_t H, int32_t W, int32_t sh_degree, float scale_modifier,
+                                       const float* views_dev, int32_t N, int32_t M, const float* means3D,
+                                       const float* shs, const float* colors_precomp, const float* opacities,
+                                       const float* scales, const float* rotations, int32_t geom_only, float* recs_out,
+                                       void* stream_) {
+    cudaStream_t s = (cudaStream_t)stream_;
+    if (V <= 0 || N <= 0 || sh_degree < 0 || sh_degree > 3 || !views_dev || !means3D || !opacities || !scales ||
+        !rotations || !recs_out || (shs == nullptr) == (colors_precomp == nullptr) || (geom_only && !shs) ||
+        (shs && (M < (sh_degree + 1) * (sh_degree + 1) || M > 16))) {
+        gs_set_error("debug_preprocess_views: bad argument"); return 1;
+    }
+    struct Regions {
+        Region r[5];
+        ~Regions() { for (Region& x : r) if (x.p) cudaFree(x.p); }
+    } R;
+    const int tiles_x = (W + GS_TILE - 1) / GS_TILE, tiles_y = (H + GS_TILE - 1) / GS_TILE;
+    const StepChunks ch(V);
+    ChunkWS w;
+    if (chunk_ws_setup(w, R.r[0], R.r[1], R.r[2], R.r[3], R.r[4], ch.VB, N, tiles_x * tiles_y,
+                       g_tile_culling.load() >= 1, s)) return 1;
+    PackedPtrs par; par.means = (float*)means3D; par.shs = (float*)shs; par.colors = (float*)colors_precomp;
+    par.opac = (float*)opacities; par.scales = (float*)scales; par.rots = (float*)rotations; par.m2d = nullptr;
+    unsigned long long host_totals[GS_MAX_SEGS];
+    for (int k = 0; k < ch.nchunks; k++) {
+        const int v0 = k * ch.VB, nv = std::min(ch.VB, V - v0);
+        const float* vchunk = views_dev + (size_t)v0 * 40;
+        if (chunk_bin_a(w, vchunk, nv, W, H, sh_degree, scale_modifier, N, M, par, geom_only ? 1 : 0, host_totals, s)) return 1;
+        if (geom_only && gs_launch_sh_colour_multi(vchunk, nv, sh_degree, N, M, par.means, par.shs, w.radii, w.recs, s)) return 1;
+        GS_CUDA_CHECK(cudaMemcpyAsync(recs_out + (size_t)v0 * N * 12, w.recs, (size_t)nv * N * sizeof(SplatRec),
+                                      cudaMemcpyDeviceToDevice, s));
+        GS_CUDA_CHECK(cudaStreamSynchronize(s));
+    }
+    return 0;
+}
+
 int32_t gs_b200_step_host(int32_t V, int32_t H, int32_t W, int32_t sh_degree, float scale_modifier,
                           const float* views_host, int32_t N, int32_t M, const float* means3D_host,
                           const float* shs_host, const float* opacities_host, const float* scales_host,

@@ -211,8 +211,10 @@ def forward_with_state(raster_settings, means3D, opacities, shs=None, colors_pre
                        rotations=None, cov3D_precomp=None):
     """Forward only, plus the binning/image state as torch tensors (parity tests, benchmarks).
 
-    Returns dict(color, radii, depth, alpha, point_list[P] int32, tile_keys[P] int32, sorted_keys[P] int64
-    (tile<<32 | float_bits(depth)), ranges[tiles,2] int32, n_contrib[H,W] int32, final_T[H,W], num_rendered).
+    Returns dict(color, radii, depth, alpha, recs[N,12] float32 (the 48-byte splat records: px, py, depth, radius bits |
+    log2-scaled conic a', b', c', opacity | r, g, b, tiles_touched bits), point_list[P] int32, tile_keys[P] int32,
+    sorted_keys[P] int64 (tile<<32 | float_bits(depth)), ranges[tiles,2] int32, n_contrib[H,W] int32, final_T[H,W],
+    num_rendered).
     """
     class _Ctx:
         def mark_non_differentiable(self, *a):
@@ -231,6 +233,9 @@ def forward_with_state(raster_settings, means3D, opacities, shs=None, colors_pre
                ranges=_view_of(bufs, st.ranges, ntiles * 2, torch.int32).view(ntiles, 2),
                n_contrib=_view_of(bufs, st.n_contrib, H * W, torch.int32).view(H, W),
                final_T=_view_of(bufs, st.final_T, H * W, torch.float32).view(H, W))
+    N = int(st.num_gaussians)
+    out["recs"] = (_view_of(bufs, st.geom, N * 12, torch.float32).view(N, 12) if N > 0 else
+                   torch.empty(0, 12, dtype=torch.float32, device=color.device))
     if P > 0:
         out["point_list"] = _view_of(bufs, st.point_list, P, torch.int32)
         out["tile_keys"] = _view_of(bufs, st.tile_keys, P, torch.int32)

@@ -174,6 +174,16 @@ int32_t gs_b200_debug_bin_views(int32_t V, int32_t H, int32_t W, int32_t sh_degr
                                 int32_t* radii, uint32_t* tiles_touched, uint32_t* spans, uint32_t* sorted_dkeys,
                                 uint32_t* sorted_ids, uint32_t* offsets, int64_t* totals, uint32_t* ranges,
                                 uint32_t* point_list, uint32_t* tile_keys, void* stream);
+/* Tests of the forward preprocess: the batched preprocess of the gs_b200_step_* entries, through the same code: views_dev
+ * [V][40] and the parameters as theirs (exactly one of shs / colors_precomp), the views in the step's chunks, tile
+ * culling as gs_b200_set_tile_culling has it for the step.  geom_only (shs only): the host-buffer step's colour-free
+ * pass, then its colour pass.  recs_out: [V][N][12] floats, the 48-byte splat records (px, py, depth, radius bits |
+ * log2-scaled conic a', b', c', opacity | r, g, b, tiles_touched bits). */
+int32_t gs_b200_debug_preprocess_views(int32_t V, int32_t H, int32_t W, int32_t sh_degree, float scale_modifier,
+                                       const float* views_dev, int32_t N, int32_t M, const float* means3D,
+                                       const float* shs, const float* colors_precomp, const float* opacities,
+                                       const float* scales, const float* rotations, int32_t geom_only, float* recs_out,
+                                       void* stream);
 /* The view chunks of the multi-view step for V views: bounds[k] is the first view of chunk k, bounds[nchunks] = V
  * (bounds holds at least V + 1 entries).  Returns nchunks, or -1 on a bad argument.  Host only. */
 int32_t gs_b200_step_view_chunks(int32_t V, int32_t* bounds);

@@ -89,7 +89,8 @@ def test_ctypes_binding_is_derived_from_every_header_in_include():
         for name, params in re.findall(r"\b((?:gs|dr|ngp)_b200_\w+)\s*\(([^()]*)\)\s*;", src):
             declared[name] = 0 if params.strip() == "void" else params.count(",") + 1
     bound = {n for n, f in vars(_lib.lib).items() if isinstance(f, _lib.lib._FuncPtr)}
-    assert len(declared) == 105 and bound == set(declared)
+    assert len(declared) == 106 and bound == set(declared)
+    assert len(_lib.lib.gs_b200_debug_preprocess_views.argtypes) == 17
     for name, nparams in declared.items():
         assert len(getattr(_lib.lib, name).argtypes) == nparams, name
 
