@@ -99,10 +99,11 @@ struct Carver {
     static size_t need(size_t count, size_t elem) { return (count * elem + 255) & ~(size_t)255; }
 };
 
-int make_view_args(const gs_b200_view* v, ViewArgs& va) {
-    if (!v || !v->bg || !v->viewmatrix || !v->projmatrix || !v->campos) { gs_set_error("view: NULL field"); return 1; }
-    if (v->image_height <= 0 || v->image_width <= 0) { gs_set_error("view: bad image size"); return 1; }
-    if (v->sh_degree < 0 || v->sh_degree > 3) { gs_set_error("view: sh_degree must be 0..3"); return 1; }
+// fn: the entry point named in the error message
+int make_view_args(const char* fn, const gs_b200_view* v, ViewArgs& va) {
+    if (!v || !v->bg || !v->viewmatrix || !v->projmatrix || !v->campos) { gs_set_error("%s: NULL view field", fn); return 1; }
+    if (v->image_height <= 0 || v->image_width <= 0) { gs_set_error("%s: bad image size", fn); return 1; }
+    if (v->sh_degree < 0 || v->sh_degree > 3) { gs_set_error("%s: sh_degree must be 0..3", fn); return 1; }
     va.view = v->viewmatrix; va.proj = v->projmatrix; va.campos = v->campos; va.bg = v->bg;
     va.tanfovx = v->tanfovx; va.tanfovy = v->tanfovy;
     va.W = v->image_width; va.H = v->image_height;
@@ -116,11 +117,13 @@ int make_view_args(const gs_b200_view* v, ViewArgs& va) {
     return 0;
 }
 
-int check_inputs(int N, int M, int sh_degree, const float* means3D, const float* shs, const float* colors_precomp,
-                 const float* opacities, const float* scales, const float* rotations, const float* cov3D_precomp) {
-    if (N < 0) { gs_set_error("N < 0"); return 1; }
+// fn: the entry point named in the error message (the package's own two messages are kept word for word)
+int check_inputs(const char* fn, int N, int M, int sh_degree, const float* means3D, const float* shs,
+                 const float* colors_precomp, const float* opacities, const float* scales, const float* rotations,
+                 const float* cov3D_precomp) {
+    if (N < 0) { gs_set_error("%s: N < 0", fn); return 1; }
     if (N == 0) return 0;      // empty cloud: pointers of empty arrays may legitimately be NULL
-    if (!means3D || !opacities) { gs_set_error("means3D/opacities NULL"); return 1; }
+    if (!means3D || !opacities) { gs_set_error("%s: means3D/opacities NULL", fn); return 1; }
     if ((shs == nullptr) == (colors_precomp == nullptr)) {
         gs_set_error("Please provide excatly one of either SHs or precomputed colors!"); return 1;
     }
@@ -128,41 +131,23 @@ int check_inputs(int N, int M, int sh_degree, const float* means3D, const float*
     if ((sr && cov3D_precomp) || (!sr && !cov3D_precomp) || (sr && (!scales || !rotations))) {
         gs_set_error("Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!"); return 1;
     }
-    if (shs && M < (sh_degree + 1) * (sh_degree + 1)) { gs_set_error("shs has %d coefficients, sh_degree %d needs %d", M, sh_degree, (sh_degree + 1) * (sh_degree + 1)); return 1; }
-    if (shs && M > 16) { gs_set_error("at most 16 SH coefficients (degree 3) supported, got %d", M); return 1; }
+    if (shs && M < (sh_degree + 1) * (sh_degree + 1)) { gs_set_error("%s: shs has %d coefficients, sh_degree %d needs %d", fn, M, sh_degree, (sh_degree + 1) * (sh_degree + 1)); return 1; }
+    if (shs && M > 16) { gs_set_error("%s: at most 16 SH coefficients (degree 3) supported, got %d", fn, M); return 1; }
     return 0;
 }
 
 // The multi-view step's view chunks: nchunks balanced chunks of <= VB views (VB <= 16, one batched preprocess, binning
-// and preprocess backward each); chunk k holds views [k VB, min(V, (k + 1) VB)).
+// and preprocess backward each); chunk k holds views [first(k), first(k) + count(k)).
 struct StepChunks {
-    int nchunks, VB;
-    explicit StepChunks(int V) {
+    int V, nchunks, VB;
+    explicit StepChunks(int V_) : V(V_) {
         const int maxv = std::min(gs_preprocess_multi_max_views(), GS_MAX_SEGS);
         nchunks = (V + maxv - 1) / maxv;
         VB = nchunks > 0 ? (V + nchunks - 1) / nchunks : 0;
     }
+    int first(int k) const { return VB * k; }
+    int count(int k) const { return std::min(VB, V - first(k)); }
 };
-
-// Preprocess backward of step chunk k (views [v0, v0 + nv)): the first chunk writes the gradients, later ones add to
-// them.  Run over `nparts` Gaussian ranges whose starts are multiples of the kernel's 128-Gaussian CTA; after(first,
-// count) follows each range's launch (a gradient sink starts the range's transfer there).
-template <class After>
-int step_backward_chunk(int k, int nparts, const float* views_chunk, int nv, int W, int H, int sh_degree,
-                        float scale_modifier, int N, int M, const float* means, const float* shs, const float* scales,
-                        const float* rots, const int32_t* radii, const SplatGrad* sg, float* gmeans, float* gm2d,
-                        float* gshs, float* gopac, float* gscales, float* grots, cudaStream_t s, After after) {
-    const int per = (((N + nparts - 1) / nparts) + 127) / 128 * 128;
-    for (int first = 0; first < N; first += per) {
-        const int count = std::min(per, N - first);
-        { StageTimer t(8, s);
-        if (gs_launch_preprocess_backward_multi(views_chunk, nv, W, H, sh_degree, scale_modifier, N, M, means, shs, scales,
-                                                rots, radii, sg, gmeans, gm2d, gshs, gopac, gscales, grots, k > 0 ? 1 : 0,
-                                                first, count, s)) return 1; }
-        after(first, count);
-    }
-    return 0;
-}
 
 int bits_for(int n) { int b = 0; while ((1 << b) < n) b++; return b < 1 ? 1 : b; }
 
@@ -196,7 +181,7 @@ static int tile_culling_init() {
 }
 static std::atomic<int> g_tile_culling{tile_culling_init()};
 int32_t gs_b200_set_tile_culling(int32_t mode) {
-    if (mode < 0 || mode > 2) { gs_set_error("tile culling mode must be 0, 1 or 2"); return 1; }
+    GS_REQ(mode >= 0 && mode <= 2, "tile culling mode must be 0, 1 or 2");
     g_tile_culling.store(mode);
     return 0;
 }
@@ -313,36 +298,25 @@ static int bin_b(const BinA& a, const ViewSpans& vs, int tiles_x, int tiles_y, c
     return 0;
 }
 
-// ---- single-view forward, split at the one host round-trip (number of (tile,splat) pairs) -----------------
-// Phase A: preprocess -> binning phase A (one view) -> async D2H of the pair count.
-// Phase B (needs P on the host to size the binning buffers): binning phase B -> composite.
-struct FwdCtx {
-    ViewArgs va; int N = 0, M = 0, dbg = 0;
-    Allocator A;
-    gs_b200_state* state = nullptr;
-    SplatRec* recs = nullptr;
-    BinA bin;
-    uint4* spans = nullptr;                        // tile culling: per-row tile spans (NULL = full squares)
-    unsigned long long* host_total = nullptr;      // pinned
-    float *out_color = nullptr, *out_depth = nullptr, *out_alpha = nullptr;
-    cudaStream_t s = nullptr;
-    FwdCtx(gs_b200_alloc_fn fn, void* user, cudaStream_t st) : A{fn, user, st}, s(st) {}
-};
-
-static int fwd_phase_a(FwdCtx& c, const gs_b200_view* view, int32_t N, int32_t M, const float* means3D,
-                       const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
-                       const float* rotations, const float* cov3D_precomp, float* out_color, float* out_depth,
-                       float* out_alpha, int32_t* radii, gs_b200_state* state, unsigned long long* host_total) {
-    cudaStream_t s = c.s;
-    if (make_view_args(view, c.va)) return 1;
-    if (check_inputs(N, M, view->sh_degree, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp)) return 1;
-    if (!out_color || !out_depth || !out_alpha || (N > 0 && !radii) || !state) { gs_set_error("forward: NULL output"); return 1; }
-    const ViewArgs& va = c.va;
-    c.N = N; c.M = M; c.dbg = view->debug; c.state = state; c.host_total = host_total;
-    c.out_color = out_color; c.out_depth = out_depth; c.out_alpha = out_alpha;
+// ---- single-view forward: preprocess -> binning phase A (one view) -> D2H of the pair count -> the one host
+// round-trip (the pair count sizes the binning buffers) -> binning phase B -> composite.
+int32_t gs_b200_rasterize_forward(const gs_b200_view* view, int32_t N, int32_t M, const float* means3D,
+                                  const float* shs, const float* colors_precomp, const float* opacities,
+                                  const float* scales, const float* rotations, const float* cov3D_precomp,
+                                  float* out_color, float* out_depth, float* out_alpha, int32_t* radii,
+                                  gs_b200_alloc_fn alloc, void* alloc_user, gs_b200_state* state, void* stream_) {
+    cudaStream_t s = (cudaStream_t)stream_;
+    ViewArgs va;
+    if (make_view_args(__func__, view, va)) return 1;
+    if (check_inputs(__func__, N, M, view->sh_degree, means3D, shs, colors_precomp, opacities, scales, rotations,
+                     cov3D_precomp)) return 1;
+    GS_REQ(out_color && out_depth && out_alpha && (N == 0 || radii) && state, "NULL output");
+    unsigned long long* host_total = pinned_u64();
+    if (!host_total) { gs_set_error("cudaHostAlloc failed"); return 1; }
+    const int dbg = view->debug;
     memset(state, 0, sizeof(*state));
     state->num_gaussians = N; state->tiles_x = va.tiles_x; state->tiles_y = va.tiles_y;
-    Allocator& A = c.A;
+    Allocator A{alloc, alloc_user, s};
     const size_t npix = (size_t)va.W * va.H;
     const int ntiles = va.tiles_x * va.tiles_y;
 
@@ -355,9 +329,11 @@ static int fwd_phase_a(FwdCtx& c, const gs_b200_view* view, int32_t N, int32_t M
     state->final_T = ci.take<float>(npix);
     GS_CUDA_CHECK(cudaMemsetAsync(state->ranges, 0, (size_t)ntiles * 2 * 4, s));
 
-    c.recs = (SplatRec*)A.get(GS_B200_BUF_GEOM, (size_t)N * sizeof(SplatRec), &state->owned[GS_B200_BUF_GEOM]);
+    SplatRec* recs = (SplatRec*)A.get(GS_B200_BUF_GEOM, (size_t)N * sizeof(SplatRec), &state->owned[GS_B200_BUF_GEOM]);
     if (A.failed) return 1;
-    state->geom = c.recs;
+    state->geom = recs;
+    BinA b;
+    uint4* spans = nullptr;                        // tile culling: per-row tile spans (NULL = full squares)
     *host_total = 0;
     if (N > 0) {
         const bool own_spans = g_tile_culling.load() == 2;
@@ -365,36 +341,27 @@ static int fwd_phase_a(FwdCtx& c, const gs_b200_view* view, int32_t N, int32_t M
         void* sc = A.get(GS_B200_BUF_SCRATCH, sc_bytes);
         if (A.failed) return 1;
         Carver cv(sc);
-        c.spans = own_spans ? cv.take<uint4>(N) : nullptr;
-        BinA& b = c.bin;
+        spans = own_spans ? cv.take<uint4>(N) : nullptr;
         b.tiles = cv.take<uint32_t>(N);
         b.dkeys = cv.take<uint32_t>(N);
         b.ids = cv.take<uint32_t>(N);
         uint32_t* min_key = (uint32_t*)cv.take<unsigned long long>(1);
         carve_bin_a(cv, b, 1, N);
-        b.minkeys = min_key; b.dbg = c.dbg;
+        b.minkeys = min_key; b.dbg = dbg;
         GS_CUDA_CHECK(cudaMemsetAsync(min_key, 0xFF, 4, s));
         { StageTimer t(0, s);
         if (gs_launch_preprocess(va, N, M, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
-                                 c.recs, radii, b.tiles, b.dkeys, b.ids, min_key, c.spans, s)) return 1; }
-        STAGE_CHECK(c.dbg, s, "preprocess");
+                                 recs, radii, b.tiles, b.dkeys, b.ids, min_key, spans, s)) return 1; }
+        STAGE_CHECK(dbg, s, "preprocess");
         if (bin_a(b, host_total, s)) return 1;
     }
-    return 0;
-}
+    GS_CUDA_CHECK(cudaStreamSynchronize(s));
 
-// caller has made sure the D2H of phase A completed (stream or event sync).  Binning half: emit -> tile sort -> ranges.
-static int fwd_phase_b_bin(FwdCtx& c) {
-    cudaStream_t s = c.s;
-    const ViewArgs& va = c.va;
-    gs_b200_state* state = c.state;
-    Allocator& A = c.A;
     ViewSpans vs;
-    if (view_spans(1, c.host_total, vs)) return 1;
+    if (view_spans(1, host_total, vs)) return 1;
     const int64_t P = vs.base[1];
     state->num_rendered = P;
-    const size_t bin_bytes = Carver::need(P, 4) * 2;
-    void* bin = A.get(GS_B200_BUF_BINNING, bin_bytes, &state->owned[GS_B200_BUF_BINNING]);
+    void* bin = A.get(GS_B200_BUF_BINNING, Carver::need(P, 4) * 2, &state->owned[GS_B200_BUF_BINNING]);
     if (A.failed) return 1;
     Carver cb(bin);
     BinB o;
@@ -405,36 +372,13 @@ static int fwd_phase_b_bin(FwdCtx& c) {
         if (A.failed) return 1;
         Carver c2(sc2);
         carve_bin_b_scratch(c2, o, 1, P);
-        if (bin_b(c.bin, vs, va.tiles_x, va.tiles_y, c.recs, c.spans, o, state->ranges, s)) return 1;
+        if (bin_b(b, vs, va.tiles_x, va.tiles_y, recs, spans, o, state->ranges, s)) return 1;
     }
-    return 0;
-}
-// composite half of phase B (the only part of the forward that reads the colours in the records)
-static int fwd_phase_b_render(FwdCtx& c) {
-    cudaStream_t s = c.s;
-    const ViewArgs& va = c.va;
-    gs_b200_state* state = c.state;
     { StageTimer t(6, s);
-    if (gs_launch_render_forward(va, c.recs, state->point_list, state->ranges, c.out_color, c.out_depth, c.out_alpha,
+    if (gs_launch_render_forward(va, recs, state->point_list, state->ranges, out_color, out_depth, out_alpha,
                                  state->n_contrib, state->final_T, s)) return 1; }
-    STAGE_CHECK(c.dbg, s, "render");
+    STAGE_CHECK(dbg, s, "render");
     return 0;
-}
-static int fwd_phase_b(FwdCtx& c) { return fwd_phase_b_bin(c) || fwd_phase_b_render(c); }
-
-int32_t gs_b200_rasterize_forward(const gs_b200_view* view, int32_t N, int32_t M, const float* means3D,
-                                  const float* shs, const float* colors_precomp, const float* opacities,
-                                  const float* scales, const float* rotations, const float* cov3D_precomp,
-                                  float* out_color, float* out_depth, float* out_alpha, int32_t* radii,
-                                  gs_b200_alloc_fn alloc, void* alloc_user, gs_b200_state* state, void* stream_) {
-    cudaStream_t s = (cudaStream_t)stream_;
-    unsigned long long* hp = pinned_u64();
-    if (!hp) { gs_set_error("cudaHostAlloc failed"); return 1; }
-    FwdCtx c(alloc, alloc_user, s);
-    if (fwd_phase_a(c, view, N, M, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
-                    out_color, out_depth, out_alpha, radii, state, hp)) return 1;
-    GS_CUDA_CHECK(cudaStreamSynchronize(s));
-    return fwd_phase_b(c);
 }
 
 int32_t gs_b200_rasterize_backward(const gs_b200_view* view, int32_t N, int32_t M, const float* means3D,
@@ -447,15 +391,14 @@ int32_t gs_b200_rasterize_backward(const gs_b200_view* view, int32_t N, int32_t 
                                    gs_b200_alloc_fn alloc, void* alloc_user, void* stream_) {
     cudaStream_t s = (cudaStream_t)stream_;
     ViewArgs va;
-    if (make_view_args(view, va)) return 1;
-    if (check_inputs(N, M, view->sh_degree, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp)) return 1;
-    if (!state || !dL_dcolor || !dL_ddepth || !dL_dalpha) { gs_set_error("backward: NULL state/upstream gradient"); return 1; }
+    if (make_view_args(__func__, view, va)) return 1;
+    if (check_inputs(__func__, N, M, view->sh_degree, means3D, shs, colors_precomp, opacities, scales, rotations,
+                     cov3D_precomp)) return 1;
+    GS_REQ(state && dL_dcolor && dL_ddepth && dL_dalpha, "NULL state/upstream gradient");
     if (N == 0) return 0;
-    if (!radii || !dL_dmeans3D || !dL_dmeans2D || !dL_dopacities || (shs && !dL_dshs) || (colors_precomp && !dL_dcolors) ||
-        (scales && (!dL_dscales || !dL_drotations)) || (cov3D_precomp && !dL_dcov3D)) {
-        gs_set_error("backward: NULL gradient output"); return 1;
-    }
-    if (state->num_gaussians != N) { gs_set_error("backward: state is for N=%d, got %d", state->num_gaussians, N); return 1; }
+    GS_REQ(radii && dL_dmeans3D && dL_dmeans2D && dL_dopacities && (!shs || dL_dshs) && (!colors_precomp || dL_dcolors) &&
+           (!scales || (dL_dscales && dL_drotations)) && (!cov3D_precomp || dL_dcov3D), "NULL gradient output");
+    if (state->num_gaussians != N) { gs_set_error("%s: state is for N=%d, got %d", __func__, state->num_gaussians, N); return 1; }
     const int dbg = view->debug;
     Allocator A{alloc, alloc_user, s};
     SplatGrad* sg = (SplatGrad*)A.get(GS_B200_BUF_SCRATCH, (size_t)N * sizeof(SplatGrad));
@@ -483,7 +426,7 @@ int32_t gs_b200_state_free(gs_b200_state* state, void* stream_) {
 }
 
 int32_t gs_b200_debug_sorted_keys(const gs_b200_state* state, uint64_t* keys_out, void* stream_) {
-    if (!state || !keys_out) { gs_set_error("debug_sorted_keys: NULL"); return 1; }
+    GS_REQ(state && keys_out, "NULL argument");
     return gs_launch_sorted_keys((const SplatRec*)state->geom, state->point_list, state->tile_keys,
                                  state->num_rendered, keys_out, (cudaStream_t)stream_);
 }
@@ -496,9 +439,10 @@ int32_t gs_b200_debug_preprocess_backward(const gs_b200_view* view, int32_t N, i
                                           float* dL_dscales, float* dL_drotations, float* dL_dcov3D, int32_t accumulate,
                                           void* stream_) {
     ViewArgs va;
-    if (make_view_args(view, va)) return 1;
-    if (check_inputs(N, M, view->sh_degree, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp)) return 1;
-    if (N > 0 && (!radii || !splat_grads)) { gs_set_error("debug_preprocess_backward: NULL radii/splat_grads"); return 1; }
+    if (make_view_args(__func__, view, va)) return 1;
+    if (check_inputs(__func__, N, M, view->sh_degree, means3D, shs, colors_precomp, opacities, scales, rotations,
+                     cov3D_precomp)) return 1;
+    GS_REQ(N == 0 || (radii && splat_grads), "NULL radii/splat_grads");
     return gs_launch_preprocess_backward(va, N, M, means3D, shs, colors_precomp, opacities, scales, rotations,
                                          cov3D_precomp, radii, (const SplatGrad*)splat_grads, dL_dmeans3D, dL_dmeans2D,
                                          dL_dshs, dL_dcolors, dL_dopacities, dL_dscales, dL_drotations, dL_dcov3D,
@@ -506,37 +450,11 @@ int32_t gs_b200_debug_preprocess_backward(const gs_b200_view* view, int32_t N, i
 }
 
 int32_t gs_b200_step_view_chunks(int32_t V, int32_t* bounds) {
-    if (V <= 0 || !bounds) { gs_set_error("step_view_chunks: bad argument"); return -1; }
+    if (V <= 0 || !bounds) { gs_set_error("%s: bad argument", __func__); return -1; }
     const StepChunks ch(V);
-    for (int k = 0; k < ch.nchunks; k++) bounds[k] = k * ch.VB;
+    for (int k = 0; k < ch.nchunks; k++) bounds[k] = ch.first(k);
     bounds[ch.nchunks] = V;
     return ch.nchunks;
-}
-
-// The preprocess backward of the multi-view step, as step_core runs it: the same chunks (StepChunks) and the same
-// per-chunk launches (step_backward_chunk), the last chunk over `nparts` Gaussian ranges as with a gradient sink.
-int32_t gs_b200_debug_preprocess_backward_multi(int32_t V, int32_t H, int32_t W, int32_t sh_degree, float scale_modifier,
-                                                const float* views_dev, int32_t N, int32_t M, const float* means3D,
-                                                const float* shs, const float* scales, const float* rotations,
-                                                const int32_t* radii, const double* splat_grads, float* grads_dev,
-                                                int32_t nparts, void* stream_) {
-    cudaStream_t s = (cudaStream_t)stream_;
-    if (V <= 0 || N <= 0 || M < (sh_degree + 1) * (sh_degree + 1) || M > 16 || nparts < 1 || !views_dev || !means3D ||
-        !shs || !scales || !rotations || !radii || !splat_grads || !grads_dev) {
-        gs_set_error("debug_preprocess_backward_multi: bad argument"); return 1;
-    }
-    // the step's gradient layout: means 3N | shs 3NM | opacities N | scales 3N | rotations 4N | means2D 3N
-    float* gm = grads_dev; float* gsh = gm + 3 * (size_t)N; float* gop = gsh + 3 * (size_t)N * M;
-    float* gsc = gop + N; float* grt = gsc + 3 * (size_t)N; float* g2 = grt + 4 * (size_t)N;
-    const SplatGrad* sg = (const SplatGrad*)splat_grads;
-    const StepChunks ch(V);
-    for (int k = 0; k < ch.nchunks; k++) {
-        const int v0 = k * ch.VB, nv = std::min(ch.VB, V - v0);
-        if (step_backward_chunk(k, k + 1 == ch.nchunks ? nparts : 1, views_dev + (size_t)v0 * 40, nv, W, H, sh_degree,
-                                scale_modifier, N, M, means3D, shs, scales, rotations, radii + (size_t)v0 * N,
-                                sg + (size_t)v0 * N, gm, g2, gsh, gop, gsc, grt, s, [](int, int) {})) return 1;
-    }
-    return 0;
 }
 
 // ---------------------------------------------------------------------------------
@@ -565,6 +483,152 @@ struct Slot {
     }
 };
 
+// The step's packed parameter and gradient buffers: six groups of N rows, means | shs | opacities | scales | rotations
+// | means2D (gradients only), of 3, 3M, 1, 3, 4 and 3 floats a row.  Group g starts at off[g]; off[5] floats hold the
+// parameters and off[6] the gradients.
+struct PackedLayout { size_t off[7], width[6]; };
+PackedLayout packed_layout(size_t N, size_t M) {
+    const size_t width[6] = {3, 3 * M, 1, 3, 4, 3};
+    PackedLayout L;
+    L.off[0] = 0;
+    for (int g = 0; g < 6; g++) { L.width[g] = width[g]; L.off[g + 1] = L.off[g] + N * width[g]; }
+    return L;
+}
+struct PackedPtrs { float *means, *shs, *opac, *scales, *rots, *m2d; float* colors = nullptr; /* [N,3] instead of shs: forward-only */ };
+PackedPtrs carve_packed(float* base, size_t N, size_t M, bool with_m2d) {
+    const PackedLayout L = packed_layout(N, M);
+    PackedPtrs p;
+    p.means = base + L.off[0]; p.shs = base + L.off[1]; p.opac = base + L.off[2]; p.scales = base + L.off[3];
+    p.rots = base + L.off[4]; p.m2d = with_m2d ? base + L.off[5] : nullptr;
+    return p;
+}
+// the parameters as the entries take them: five arrays (and, for a forward-only caller, precomputed colours)
+PackedPtrs param_ptrs(const float* means, const float* shs, const float* opac, const float* scales, const float* rots,
+                      const float* colors = nullptr) {
+    PackedPtrs p;
+    p.means = (float*)means; p.shs = (float*)shs; p.opac = (float*)opac; p.scales = (float*)scales; p.rots = (float*)rots;
+    p.m2d = nullptr; p.colors = (float*)colors;
+    return p;
+}
+
+// Gradient sink: fn(user, first, count, stream) is called after each Gaussian range [first, first + count) of the
+// step's LAST preprocess-backward has been enqueued on `stream`; that pass runs over nchunks such ranges.
+struct GradSink { gs_b200_grad_sink fn = nullptr; void* user = nullptr; int nchunks = 1; };
+thread_local GradSink g_grad_sink;       // gs_b200_set_grad_sink: a data-parallel caller's all-reduce
+
+// What every view chunk of one multi-view step shares: the views (views_dev: [V][40] floats, in chunks ch), image and
+// SH sizes, and the parameters.  geom_only: the preprocess leaves the records' colours to a pass after the binning,
+// which first waits for shs_ready (if set): the host-buffer step's SH block is still being uploaded.
+struct StepScene {
+    StepChunks ch;
+    const float* views_dev;
+    int W, H, tiles_x, tiles_y, sh_degree;
+    float scale_modifier;
+    int N, M;
+    PackedPtrs par;
+    bool geom_only;
+    cudaEvent_t shs_ready;
+    StepScene(int V, int H_, int W_, int sh_degree_, float scale_modifier_, const float* views_dev_, int N_, int M_,
+              const PackedPtrs& par_, bool geom_only_ = false, cudaEvent_t shs_ready_ = nullptr)
+        : ch(V), views_dev(views_dev_), W(W_), H(H_), tiles_x((W_ + GS_TILE - 1) / GS_TILE),
+          tiles_y((H_ + GS_TILE - 1) / GS_TILE), sh_degree(sh_degree_), scale_modifier(scale_modifier_), N(N_), M(M_),
+          par(par_), geom_only(geom_only_), shs_ready(shs_ready_) {}
+    const float* views(int k) const { return views_dev + (size_t)ch.first(k) * 40; }
+};
+
+size_t chunk_pairs_bytes(int nv, int64_t P) { return Carver::need(P, 4) * 2 + bin_b_scratch_bytes(nv, P); }
+
+// Workspace of one view chunk of the multi-view step, in six grow-only regions that are freed with it: [VB][N]
+// preprocess outputs and depth sort, the binning scratch and [VB][tiles][2] ranges, and the chunk's pair lists.
+struct ChunkWS {
+    Region r_recs, r_sg, r_u32, r_spans, r_bin, r_pairs;
+    SplatRec* recs; SplatGrad* sg; int32_t* radii; uint32_t *minkeys, *ranges; uint4* spans; BinA bin;
+    ViewSpans vs; BinB pairs;           // the chunk's per-view pair bases and pair lists (chunk_bin)
+
+    ChunkWS() = default;
+    ChunkWS(const ChunkWS&) = delete;
+    ChunkWS& operator=(const ChunkWS&) = delete;
+    ~ChunkWS() {
+        for (Region* r : {&r_recs, &r_sg, &r_u32, &r_spans, &r_bin, &r_pairs}) if (r->p) cudaFree(r->p);
+    }
+    // sized for the scene's largest chunk; tight: with the tile culling's spans
+    int setup(const StepScene& sc, bool tight, cudaStream_t s) {
+        const int VB = sc.ch.VB, ntiles = sc.tiles_x * sc.tiles_y;
+        const size_t nvb = (size_t)VB * sc.N;
+        if (Slot::ensure(r_recs, nvb * sizeof(SplatRec), s) || Slot::ensure(r_sg, nvb * sizeof(SplatGrad), s) ||
+            Slot::ensure(r_u32, nvb * 4 * 4 + 256 * 4, s) ||
+            Slot::ensure(r_bin, bin_a_bytes(VB, sc.N) + Carver::need((size_t)VB * ntiles * 2, 4), s)) return 1;
+        if (tight && Slot::ensure(r_spans, nvb * sizeof(uint4), s)) return 1;
+        uint32_t* u32 = (uint32_t*)r_u32.p;
+        recs = (SplatRec*)r_recs.p; sg = (SplatGrad*)r_sg.p; radii = (int32_t*)u32;
+        minkeys = u32 + 4 * nvb;        // [VB] stride 2 words
+        spans = tight ? (uint4*)r_spans.p : nullptr;
+        bin.tiles = u32 + nvb; bin.dkeys = u32 + 2 * nvb; bin.ids = u32 + 3 * nvb;
+        bin.minkeys = minkeys; bin.minkey_stride = 2;
+        Carver cb(r_bin.p);
+        ranges = cb.take<uint32_t>((size_t)VB * ntiles * 2);
+        carve_bin_a(cb, bin, VB, sc.N);
+        return 0;
+    }
+};
+
+// ---- the three per-chunk stages of the multi-view step.  step_core runs them on its aux stream; the test entries run
+// them on one stream.
+// Projection of chunk k: preprocess, depth sort, scan, and the D2H of the views' pair counts to host_totals.
+int chunk_project(ChunkWS& w, const StepScene& sc, int k, unsigned long long* host_totals, cudaStream_t s) {
+    const PackedPtrs& p = sc.par;
+    const int nv = sc.ch.count(k);
+    GS_CUDA_CHECK(cudaMemsetAsync(w.minkeys, 0xFF, 256 * 4, s));
+    { StageTimer t(0, s);
+    if (gs_launch_preprocess_multi(sc.views(k), nv, sc.W, sc.H, sc.sh_degree, sc.scale_modifier, sc.N, sc.M, p.means,
+                                   p.shs, p.colors, p.opac, p.scales, p.rots, w.recs, w.radii, w.bin.tiles, w.bin.dkeys,
+                                   w.bin.ids, w.minkeys, w.spans, s, sc.geom_only ? 1 : 0)) return 1; }
+    w.bin.nv = nv;
+    return bin_a(w.bin, host_totals, s);
+}
+// Binning of chunk k, once host_totals holds its pair counts: the per-view pair bases (view_spans), the pair lists in
+// the grow-only pairs region (fill_pairs: pre-filled with 0xFF bytes, so a slot the emit leaves unwritten reads
+// 0xFFFFFFFF after the sort), ranges, emit, tile sort; then, for a geom_only scene, the records' colours.
+int chunk_bin(ChunkWS& w, const StepScene& sc, int k, const unsigned long long* host_totals, bool fill_pairs,
+              cudaStream_t s) {
+    const int nv = sc.ch.count(k);
+    if (view_spans(nv, host_totals, w.vs)) return 1;
+    const int64_t P = w.vs.base[nv];
+    const size_t bytes = chunk_pairs_bytes(nv, P);
+    if (Slot::ensure(w.r_pairs, bytes, s)) return 1;
+    if (fill_pairs) GS_CUDA_CHECK(cudaMemsetAsync(w.r_pairs.p, 0xFF, bytes, s));
+    Carver cp(w.r_pairs.p);
+    w.pairs.point_list = cp.take<uint32_t>(P); w.pairs.tile_keys = cp.take<uint32_t>(P);
+    carve_bin_b_scratch(cp, w.pairs, nv, P);
+    GS_CUDA_CHECK(cudaMemsetAsync(w.ranges, 0, (size_t)nv * sc.tiles_x * sc.tiles_y * 2 * 4, s));
+    if (bin_b(w.bin, w.vs, sc.tiles_x, sc.tiles_y, w.recs, w.spans, w.pairs, w.ranges, s)) return 1;
+    if (sc.geom_only) {
+        if (sc.shs_ready) GS_CUDA_CHECK(cudaStreamWaitEvent(s, sc.shs_ready, 0));
+        const PackedPtrs& p = sc.par;
+        if (gs_launch_sh_colour_multi(sc.views(k), nv, sc.sh_degree, sc.N, sc.M, p.means, p.shs, w.radii, w.recs, s)) return 1;
+    }
+    return 0;
+}
+// Preprocess backward of chunk k from its views' [count(k)][N] radii and SplatGrad: the first chunk writes the
+// gradients grd, later ones add to them.  Run over `nparts` Gaussian ranges whose starts are multiples of the kernel's
+// 128-Gaussian CTA; the sink (optional) follows each range's launch.
+int chunk_backward(const StepScene& sc, int k, const int32_t* radii, const SplatGrad* sg, const PackedPtrs& grd,
+                   int nparts, const GradSink* sink, cudaStream_t s) {
+    const PackedPtrs& p = sc.par;
+    const int N = sc.N;
+    const int per = (((N + nparts - 1) / nparts) + 127) / 128 * 128;
+    for (int first = 0; first < N; first += per) {
+        const int count = std::min(per, N - first);
+        { StageTimer t(8, s);
+        if (gs_launch_preprocess_backward_multi(sc.views(k), sc.ch.count(k), sc.W, sc.H, sc.sh_degree, sc.scale_modifier,
+                                                N, sc.M, p.means, p.shs, p.scales, p.rots, radii, sg, grd.means, grd.m2d,
+                                                grd.shs, grd.opac, grd.scales, grd.rots, k > 0 ? 1 : 0, first, count,
+                                                s)) return 1; }
+        if (sink) sink->fn(sink->user, first, count, (void*)s);
+    }
+    return 0;
+}
+
 constexpr int NSLOTS = 2;       // the composites of a chunk's views alternate between two slot streams
 struct StepCache {
     Slot slot[NSLOTS];
@@ -576,9 +640,7 @@ struct StepCache {
     std::vector<cudaEvent_t> up_ready;          // per view: upstream gradient resident
     Region host_stage;                           // device copies of host inputs (step_host)
     bool busy = false;                           // a view hook must not re-enter the step entries on this thread
-    // per-chunk workspaces of the multi-view step, two sets that alternate between chunks: [VB][N] arrays of the
-    // preprocess and the depth sort, the binning scratch and ranges, and the chunk's pair lists
-    Region ws_recs[2], ws_sg[2], ws_u32[2], ws_spans[2], ws_bin[2], ws_pairs[2];
+    ChunkWS ws[2];                               // two chunk workspaces that alternate between chunks
     int ensure_init() {
         if (init) return 0;
         for (int i = 0; i < NSLOTS; i++) {
@@ -612,61 +674,6 @@ StepCache& step_cache() {
     if (!caches[dev]) caches[dev].reset(new StepCache());
     return *caches[dev];
 }
-struct UserSink { gs_b200_grad_sink fn = nullptr; void* user = nullptr; int nchunks = 1; };
-thread_local UserSink g_user_sink;
-
-struct PackedPtrs { float *means, *shs, *opac, *scales, *rots, *m2d; float* colors = nullptr; /* [N,3] instead of shs: forward-only */ };
-PackedPtrs carve_packed(float* base, size_t N, size_t M, bool with_m2d) {
-    PackedPtrs p;
-    p.means = base; p.shs = p.means + N * 3; p.opac = p.shs + N * 3 * M; p.scales = p.opac + N;
-    p.rots = p.scales + N * 3; p.m2d = with_m2d ? p.rots + N * 4 : nullptr;
-    return p;
-}
-
-// Workspace of one view chunk of the multi-view step: [VB][N] preprocess outputs and depth sort, binning scratch and
-// [VB][tiles][2] ranges, in five grow-only regions.
-struct ChunkWS { SplatRec* recs; SplatGrad* sg; int32_t* radii; uint32_t *minkeys, *ranges; uint4* spans; BinA bin; };
-int chunk_ws_setup(ChunkWS& w, Region& r_recs, Region& r_sg, Region& r_u32, Region& r_spans, Region& r_bin, int VB, int N,
-                   int ntiles, bool tight, cudaStream_t s) {
-    const size_t nvb = (size_t)VB * N;
-    if (Slot::ensure(r_recs, nvb * sizeof(SplatRec), s) || Slot::ensure(r_sg, nvb * sizeof(SplatGrad), s) ||
-        Slot::ensure(r_u32, nvb * 4 * 4 + 256 * 4, s) ||
-        Slot::ensure(r_bin, bin_a_bytes(VB, N) + Carver::need((size_t)VB * ntiles * 2, 4), s)) return 1;
-    if (tight && Slot::ensure(r_spans, nvb * sizeof(uint4), s)) return 1;
-    uint32_t* u32 = (uint32_t*)r_u32.p;
-    w.recs = (SplatRec*)r_recs.p; w.sg = (SplatGrad*)r_sg.p; w.radii = (int32_t*)u32;
-    w.minkeys = u32 + 4 * nvb;        // [VB] stride 2 words
-    w.spans = tight ? (uint4*)r_spans.p : nullptr;
-    w.bin.tiles = u32 + nvb; w.bin.dkeys = u32 + 2 * nvb; w.bin.ids = u32 + 3 * nvb;
-    w.bin.minkeys = w.minkeys; w.bin.minkey_stride = 2;
-    Carver cb(r_bin.p);
-    w.ranges = cb.take<uint32_t>((size_t)VB * ntiles * 2);
-    carve_bin_a(cb, w.bin, VB, N);
-    return 0;
-}
-// First half of a chunk's projection and binning (views_chunk: its nv views): preprocess, depth sort, scan, and the
-// D2H of the views' pair counts to host_totals.  geom_only: colours follow from gs_launch_sh_colour_multi.
-int chunk_bin_a(ChunkWS& w, const float* views_chunk, int nv, int W, int H, int sh_degree, float scale_modifier, int N,
-                int M, const PackedPtrs& par, int geom_only, unsigned long long* host_totals, cudaStream_t s) {
-    GS_CUDA_CHECK(cudaMemsetAsync(w.minkeys, 0xFF, 256 * 4, s));
-    { StageTimer t(0, s);
-    if (gs_launch_preprocess_multi(views_chunk, nv, W, H, sh_degree, scale_modifier, N, M, par.means, par.shs, par.colors,
-                                   par.opac, par.scales, par.rots, w.recs, w.radii, w.bin.tiles, w.bin.dkeys, w.bin.ids,
-                                   w.minkeys, w.spans, s, geom_only)) return 1; }
-    w.bin.nv = nv;
-    return bin_a(w.bin, host_totals, s);
-}
-size_t chunk_pairs_bytes(int nv, int64_t P) { return Carver::need(P, 4) * 2 + bin_b_scratch_bytes(nv, P); }
-// Second half, once the host has the chunk's pair bases vs (view_spans): the pair lists o carved from `pairs`
-// (chunk_pairs_bytes), ranges, emit, tile sort.
-int chunk_bin_b(ChunkWS& w, const ViewSpans& vs, void* pairs, BinB& o, int tiles_x, int tiles_y, cudaStream_t s) {
-    const int64_t P = vs.base[vs.n];
-    Carver cp(pairs);
-    o.point_list = cp.take<uint32_t>(P); o.tile_keys = cp.take<uint32_t>(P);
-    carve_bin_b_scratch(cp, o, vs.n, P);
-    GS_CUDA_CHECK(cudaMemsetAsync(w.ranges, 0, (size_t)vs.n * tiles_x * tiles_y * 2 * 4, s));
-    return bin_b(w.bin, vs, tiles_x, tiles_y, w.recs, w.spans, o, w.ranges, s);
-}
 
 // Device-resident core.  views_host gives tanfov per view (host side), views_dev the matrices.
 // Views are handled in chunks of <= VB.  Per chunk, on the aux stream: ONE multi-view preprocess pass over the
@@ -674,89 +681,58 @@ int chunk_bin_b(ChunkWS& w, const ViewSpans& vs, void* pairs, BinB& o, int tiles
 // one host wait for the pair counts, emit, segmented tile sort, ranges).  Then per view, on the slot streams:
 // composite forward -> view hook -> SplatGrad zeroing -> composite backward.  Then ONE multi-view
 // preprocess-backward pass (parameters read once, gradients written once).
-// grad_sink (optional): called after each Gaussian range [first, first+count) of the FINAL preprocess-backward has
-// been enqueued on `user`, so a host-buffer caller can start the D2H of that range while the next one computes.
-struct GradSink { void (*fn)(void* ctx, int first, int count, cudaStream_t user); void* ctx; int nchunks; };
 // view hook (optional): called on the host after view v's forward has been enqueued on its slot stream and before
 // its backward is; the callee enqueues, on that stream, whatever turns images[v] into dL_dout[v] (the loss).
 // forward_only: no backward at all (render entry).  radii_out (optional): [V][N] per-view radii.
 // shs_ready (optional, host-buffer step): the SH block is still being uploaded when the step starts -- `user` is ordered
 // after the geometry parameters only.  Projection and binning of each chunk run first (colour-free), the colours are
 // filled in when the event fires (sh_colour_multi on the aux stream), then the composites follow.
+// sink (optional): follows the ranges of the final preprocess-backward (the host-buffer step starts the D2H of each
+// range there while the next one computes); without one, the sink set by gs_b200_set_grad_sink, if any.
 struct StepOpts { gs_b200_view_hook hook = nullptr; void* hook_user = nullptr; bool forward_only = false; int32_t* radii_out = nullptr;
-                  cudaEvent_t shs_ready = nullptr; };
+                  cudaEvent_t shs_ready = nullptr; GradSink sink; };
 
 int step_core(int V, int H, int W, int sh_degree, float scale_modifier, const float* views_host,
               const float* views_dev, int N, int M, const PackedPtrs& par, const float* dL_dout_dev,
               const cudaEvent_t* up_ready, const PackedPtrs& grd, float* images_dev, int64_t* num_rendered_out,
-              cudaStream_t user, const GradSink* sink = nullptr, const StepOpts* opts = nullptr) {
+              cudaStream_t user, const StepOpts& O = StepOpts()) {
     StepCache& C = step_cache();
     if (C.busy) { gs_set_error("step: re-entrant call from a view hook (the per-thread pipeline state is in use)"); return 1; }
     struct BusyGuard { bool& b; explicit BusyGuard(bool& x) : b(x) { b = true; } ~BusyGuard() { b = false; } } busy_guard(C.busy);
-    const StepOpts defaults;
-    const StepOpts& O = opts ? *opts : defaults;
     if (C.ensure_init()) return 1;
-    GradSink user_sink;
-    if (!sink && g_user_sink.fn && !O.forward_only) {      // data-parallel caller: all-reduce chunks behind the last pass
-        user_sink.ctx = &g_user_sink;
-        user_sink.nchunks = g_user_sink.nchunks;
-        user_sink.fn = [](void* vp, int first, int count, cudaStream_t st) {
-            UserSink* u = (UserSink*)vp;
-            u->fn(u->user, first, count, (void*)st);
-        };
-        sink = &user_sink;
-    }
+    const GradSink& sink = O.sink.fn ? O.sink : g_grad_sink;
     const size_t npix = (size_t)H * W;
-    const int tiles_x = (W + GS_TILE - 1) / GS_TILE, tiles_y = (H + GS_TILE - 1) / GS_TILE, ntiles = tiles_x * tiles_y;
     // View chunks: one batched preprocess + binning / preprocess-backward per chunk of <= 16 views, on the aux stream:
     //   aux stream:   pre+bin(0) | pre+bin(1) ......... bwd(0) | pre+bin(2) ...... bwd(1) | ... | bwd(last)
     //   slot streams:             views of chunk 0 ............. views of chunk 1 .......
     // pre+bin(k+1) is enqueued when chunk k's views start (its second half, after the host has read the pair counts,
     // once they have all been enqueued), bwd(k) after that; two workspace sets alternate and the aux stream's own
     // order (bwd(k-1) before pre(k+1)) protects their reuse.
-    const StepChunks chunks(V);
-    const int nchunks = chunks.nchunks, VB = chunks.VB;
-    const bool tight = g_tile_culling.load() >= 1;
     const bool late = O.shs_ready && par.shs && !par.colors;
+    const StepScene sc(V, H, W, sh_degree, scale_modifier, views_dev, N, M, par, late, late ? O.shs_ready : nullptr);
+    const int nchunks = sc.ch.nchunks, ntiles = sc.tiles_x * sc.tiles_y;
+    const bool tight = g_tile_culling.load() >= 1;
     if (O.shs_ready && !late) GS_CUDA_CHECK(cudaStreamWaitEvent(user, O.shs_ready, 0));
-    ChunkWS ws[2];
     const int nsets = nchunks > 1 ? 2 : 1;
     for (int i = 0; i < nsets; i++)
-        if (chunk_ws_setup(ws[i], C.ws_recs[i], C.ws_sg[i], C.ws_u32[i], C.ws_spans[i], C.ws_bin[i], VB, N, ntiles, tight,
-                           user)) return 1;
+        if (C.ws[i].setup(sc, tight, user)) return 1;
     cudaStream_t aux = C.aux_stream;
     // everything is ordered after the caller's stream
     GS_CUDA_CHECK(cudaEventRecord(C.evFork, user));
     GS_CUDA_CHECK(cudaStreamWaitEvent(aux, C.evFork, 0));
 
     int64_t rendered = 0;
-    ViewSpans vsp[2];
-    BinB pairs[2];
-    // first half of chunk k's projection and binning on the aux stream: preprocess, depth sort, scan, pair counts D2H
     auto enqueue_pre = [&](int k) -> int {
-        const int v0 = k * VB, nv = std::min(VB, V - v0);
-        if (chunk_bin_a(ws[k & (nsets - 1)], views_dev + (size_t)v0 * 40, nv, W, H, sh_degree, scale_modifier, N, M, par,
-                        late ? 1 : 0, C.host_totals[k & 1], aux)) return 1;
+        if (chunk_project(C.ws[k & (nsets - 1)], sc, k, C.host_totals[k & 1], aux)) return 1;
         GS_CUDA_CHECK(cudaEventRecord(C.evBinA[k & 1], aux));
         return 0;
     };
-    // second half, once the chunk's pair counts are on the host: pair buffers, emit, tile sort, ranges (+ colours)
     auto enqueue_bin = [&](int k) -> int {
-        const int v0 = k * VB, nv = std::min(VB, V - v0);
-        const int q = k & (nsets - 1);
-        ChunkWS& w = ws[q];
+        ChunkWS& w = C.ws[k & (nsets - 1)];
         GS_CUDA_CHECK(cudaEventSynchronize(C.evBinA[k & 1]));
-        ViewSpans& vs = vsp[k & 1];
-        if (view_spans(nv, C.host_totals[k & 1], vs)) return 1;
-        const int64_t P = vs.base[nv];
-        rendered += P;
         // grow-only: the pair lists of all the chunk's views live until its last composite backward
-        if (Slot::ensure(C.ws_pairs[q], chunk_pairs_bytes(nv, P), aux)) return 1;
-        if (chunk_bin_b(w, vs, C.ws_pairs[q].p, pairs[k & 1], tiles_x, tiles_y, aux)) return 1;
-        if (late) {
-            GS_CUDA_CHECK(cudaStreamWaitEvent(aux, O.shs_ready, 0));
-            if (gs_launch_sh_colour_multi(views_dev + (size_t)v0 * 40, nv, sh_degree, N, M, par.means, par.shs, w.radii, w.recs, aux)) return 1;
-        }
+        if (chunk_bin(w, sc, k, C.host_totals[k & 1], false, aux)) return 1;
+        rendered += w.vs.base[w.vs.n];
         GS_CUDA_CHECK(cudaEventRecord(C.evBin[k & 1], aux));
         return 0;
     };
@@ -764,10 +740,8 @@ int step_core(int V, int H, int W, int sh_degree, float scale_modifier, const fl
     int rc = enqueue_pre(0);
     if (!rc) rc = enqueue_bin(0);
     for (int k = 0; k < nchunks && !rc; k++) {
-        const int v0 = k * VB, nv = std::min(VB, V - v0);
-        const ChunkWS& w = ws[k & (nsets - 1)];
-        const ViewSpans& vs = vsp[k & 1];
-        const BinB& o = pairs[k & 1];
+        const int v0 = sc.ch.first(k), nv = sc.ch.count(k);
+        const ChunkWS& w = C.ws[k & (nsets - 1)];
         // the slot streams continue after this chunk's binning ...
         for (int i = 0; i < NSLOTS; i++) GS_CUDA_CHECK(cudaStreamWaitEvent(C.slot[i].stream, C.evBin[k & 1], 0));
         // ... while the next chunk's preprocess and depth sort already run beside them
@@ -785,14 +759,14 @@ int step_core(int V, int H, int W, int sh_degree, float scale_modifier, const fl
             vw.bg = vd + 35; vw.scale_modifier = scale_modifier; vw.viewmatrix = vd; vw.projmatrix = vd + 16;
             vw.sh_degree = sh_degree; vw.campos = vd + 32; vw.prefiltered = 0; vw.debug = 0;
             ViewArgs va;
-            if ((rc = make_view_args(&vw, va))) break;
+            if ((rc = make_view_args("step", &vw, va))) break;
             float* img = images_dev ? images_dev + (size_t)v * 5 * npix : (float*)S.image.p;
             Carver cn(S.nc.p);
             uint32_t* n_contrib = cn.take<uint32_t>(npix);
             float* final_T = cn.take<float>(npix);
             const size_t off = (size_t)j * N;
             const SplatRec* recs = w.recs + off;
-            const uint32_t* point_list = o.point_list + vs.base[j];
+            const uint32_t* point_list = w.pairs.point_list + w.vs.base[j];
             const uint32_t* ranges = w.ranges + (size_t)j * ntiles * 2;
             { StageTimer t(6, S.stream);
             if ((rc = gs_launch_render_forward(va, recs, point_list, ranges, img, img + 3 * npix, img + 4 * npix,
@@ -805,7 +779,7 @@ int step_core(int V, int H, int W, int sh_degree, float scale_modifier, const fl
             // composites.  Also for a view without pairs, whose composite backward is skipped: the batched
             // preprocess-backward reads the slice for every Gaussian with radii > 0.
             GS_CUDA_CHECK(cudaMemsetAsync(w.sg + off, 0, (size_t)N * sizeof(SplatGrad), S.stream));
-            if (vs.base[j + 1] > vs.base[j]) {
+            if (w.vs.base[j + 1] > w.vs.base[j]) {
                 StageTimer t(7, S.stream);
                 if ((rc = gs_launch_render_backward(va, recs, point_list, ranges, n_contrib, final_T, up, up + 3 * npix,
                                                     up + 4 * npix, w.sg + off, S.stream))) break;
@@ -821,13 +795,8 @@ int step_core(int V, int H, int W, int sh_degree, float scale_modifier, const fl
         if (rc) break;
         if (O.radii_out) GS_CUDA_CHECK(cudaMemcpyAsync(O.radii_out + (size_t)v0 * N, w.radii, (size_t)nv * N * 4, cudaMemcpyDeviceToDevice, aux));
         if (O.forward_only) continue;
-        const bool last_chunk = k + 1 == nchunks;
-        const int nparts = (sink && last_chunk && sink->nchunks > 1) ? sink->nchunks : 1;
-        rc = step_backward_chunk(k, nparts, views_dev + (size_t)v0 * 40, nv, W, H, sh_degree, scale_modifier, N, M,
-                                 par.means, par.shs, par.scales, par.rots, w.radii, w.sg, grd.means, grd.m2d, grd.shs,
-                                 grd.opac, grd.scales, grd.rots, aux, [&](int first, int count) {
-                                     if (sink && last_chunk) sink->fn(sink->ctx, first, count, aux);
-                                 });
+        const GradSink* last = k + 1 == nchunks && sink.fn ? &sink : nullptr;       // the sink follows the last pass
+        rc = chunk_backward(sc, k, w.radii, w.sg, grd, last ? last->nchunks : 1, last, aux);
     }
     // join: the caller's stream continues after the aux stream (which has waited for both slot streams)
     for (int i = 0; i < NSLOTS; i++) {          // (on an error path the slots may not have been joined into aux yet)
@@ -840,19 +809,20 @@ int step_core(int V, int H, int W, int sh_degree, float scale_modifier, const fl
     return rc;
 }
 
-int step_host_impl(int32_t V, int32_t H, int32_t W, int32_t sh_degree, float scale_modifier,
+// fn: the entry point named in the error message
+int step_host_impl(const char* fn, int32_t V, int32_t H, int32_t W, int32_t sh_degree, float scale_modifier,
                    const float* views_host, int32_t N, int32_t M, const float* means3D_host,
                    const float* shs_host, const float* opacities_host, const float* scales_host,
                    const float* rotations_host, const float* dL_dout_host, float* grads_host, float* grads_dev,
                    float* images_host, int64_t* num_rendered_out, void* stream_) {
     cudaStream_t s = (cudaStream_t)stream_;
     if (V <= 0 || N <= 0 || !views_host || !means3D_host || !shs_host || !opacities_host || !scales_host ||
-        !rotations_host || !dL_dout_host || (!grads_host && !grads_dev)) { gs_set_error("step_host: bad argument"); return 1; }
+        !rotations_host || !dL_dout_host || (!grads_host && !grads_dev)) { gs_set_error("%s: bad argument", fn); return 1; }
     StepCache& C = step_cache();
     if (C.ensure_init()) return 1;
     const size_t npix = (size_t)H * W;
-    const size_t n_par = (size_t)N * (3 + 3 * (size_t)M + 1 + 3 + 4);
-    const size_t n_grad = n_par + (size_t)N * 3;
+    const PackedLayout L = packed_layout(N, M);
+    const size_t n_par = L.off[5], n_grad = L.off[6];
     const size_t need = Carver::need(n_par, 4) + Carver::need(n_grad, 4) + Carver::need((size_t)V * 40, 4) +
                         Carver::need((size_t)V * 5 * npix, 4) * (images_host ? 2 : 1);
     if (Slot::ensure(C.host_stage, need, s)) return 1;
@@ -888,27 +858,25 @@ int step_host_impl(int32_t V, int32_t H, int32_t W, int32_t sh_degree, float sca
     GS_CUDA_CHECK(cudaStreamWaitEvent(s, C.evGeom, 0));
     StepOpts opts;
     opts.shs_ready = C.evPB;
-    // D2H of the summed gradients is chunked over Gaussian ranges and starts as soon as a range is final
-    struct SinkCtx { StepCache* C; float* host; float* dev; size_t N, M; } sctx{&C, grads_host, d_grad, (size_t)N, (size_t)M};
-    GradSink sink;
-    sink.ctx = &sctx; sink.nchunks = grads_host ? 4 : 1;
-    sink.fn = [](void* vp, int first, int count, cudaStream_t user) {
+    // D2H of the summed gradients is chunked over Gaussian ranges and starts as soon as a range is final.  The sink is
+    // set with device gradients too (it then copies nothing), so a sink from gs_b200_set_grad_sink never applies here.
+    struct SinkCtx { StepCache* C; float* host; float* dev; PackedLayout L; } sctx{&C, grads_host, d_grad, L};
+    opts.sink.user = &sctx;
+    opts.sink.nchunks = grads_host ? 4 : 1;
+    opts.sink.fn = [](void* vp, int32_t first, int32_t count, void* st) {
         SinkCtx* q = (SinkCtx*)vp;
         if (!q->host) return;
         StepCache& C2 = *q->C;
-        cudaEventRecord(C2.evD2H, user);
+        cudaEventRecord(C2.evD2H, (cudaStream_t)st);
         cudaStreamWaitEvent(C2.d2h_stream, C2.evD2H, 0);
-        const size_t n = q->N, M2 = q->M;
-        const size_t goff[6] = {0, 3 * n, 3 * n + 3 * M2 * n, 3 * n + 3 * M2 * n + n, 3 * n + 3 * M2 * n + 4 * n, 3 * n + 3 * M2 * n + 8 * n};
-        const size_t per[6] = {3, 3 * M2, 1, 3, 4, 3};          // means | shs | opac | scales | rots | means2D
-        for (int gI = 0; gI < 6; gI++) {
-            const size_t off = goff[gI] + (size_t)first * per[gI];
-            cudaMemcpyAsync(q->host + off, q->dev + off, (size_t)count * per[gI] * 4, cudaMemcpyDeviceToHost, C2.d2h_stream);
+        for (int g = 0; g < 6; g++) {
+            const size_t off = q->L.off[g] + (size_t)first * q->L.width[g];
+            cudaMemcpyAsync(q->host + off, q->dev + off, (size_t)count * q->L.width[g] * 4, cudaMemcpyDeviceToHost, C2.d2h_stream);
         }
     };
     // no memset of the gradient buffer: the first view chunk's preprocess-backward writes every element (accumulate = 0)
     if (step_core(V, H, W, sh_degree, scale_modifier, views_host, d_views, N, M, par, d_up, C.up_ready.data(), grd,
-                  d_img, num_rendered_out, s, &sink, &opts)) return 1;
+                  d_img, num_rendered_out, s, opts)) return 1;
     if (grads_dev) GS_CUDA_CHECK(cudaMemcpyAsync(grads_dev, d_grad, n_grad * 4, cudaMemcpyDeviceToDevice, s));
     if (images_host) GS_CUDA_CHECK(cudaMemcpyAsync(images_host, d_img, (size_t)V * 5 * npix * 4, cudaMemcpyDeviceToHost, s));
     if (grads_host) GS_CUDA_CHECK(cudaStreamSynchronize(C.d2h_stream));
@@ -918,8 +886,8 @@ int step_host_impl(int32_t V, int32_t H, int32_t W, int32_t sh_degree, float sca
 }  // namespace
 
 int32_t gs_b200_set_grad_sink(gs_b200_grad_sink sink, void* user, int32_t nchunks) {
-    if (sink && (nchunks < 1 || nchunks > 64)) { gs_set_error("set_grad_sink: nchunks must be 1..64"); return 1; }
-    g_user_sink.fn = sink; g_user_sink.user = user; g_user_sink.nchunks = sink ? nchunks : 1;
+    GS_REQ(!sink || (nchunks >= 1 && nchunks <= 64), "nchunks must be 1..64");
+    g_grad_sink.fn = sink; g_grad_sink.user = user; g_grad_sink.nchunks = sink ? nchunks : 1;
     return 0;
 }
 
@@ -928,16 +896,12 @@ int32_t gs_b200_step_device(int32_t V, int32_t H, int32_t W, int32_t sh_degree, 
                             const float* means3D, const float* shs, const float* opacities, const float* scales,
                             const float* rotations, const float* dL_dout, float* grads, float* images,
                             int64_t* num_rendered_out, void* stream_) {
-    cudaStream_t s = (cudaStream_t)stream_;
-    if (V <= 0 || N <= 0 || !views_host || !views_dev || !means3D || !shs || !opacities || !scales || !rotations ||
-        !dL_dout || !grads) { gs_set_error("step_device: bad argument"); return 1; }
-    PackedPtrs par; par.means = (float*)means3D; par.shs = (float*)shs; par.opac = (float*)opacities;
-    par.scales = (float*)scales; par.rots = (float*)rotations; par.m2d = nullptr;
-    const size_t n_grad = (size_t)N * (3 + 3 * (size_t)M + 1 + 3 + 4) + (size_t)N * 3;
-    (void)n_grad;   // grads need no memset: the first chunk's preprocess-backward writes every element
-    const PackedPtrs grd = carve_packed(grads, N, M, true);
-    return step_core(V, H, W, sh_degree, scale_modifier, views_host, views_dev, N, M, par, dL_dout, nullptr, grd, images,
-                     num_rendered_out, s);
+    GS_REQ(V > 0 && N > 0 && views_host && views_dev && means3D && shs && opacities && scales && rotations && dL_dout &&
+           grads, "bad argument");
+    // grads need no memset: the first chunk's preprocess-backward writes every element
+    return step_core(V, H, W, sh_degree, scale_modifier, views_host, views_dev, N, M,
+                     param_ptrs(means3D, shs, opacities, scales, rotations), dL_dout, nullptr,
+                     carve_packed(grads, N, M, true), images, num_rendered_out, (cudaStream_t)stream_);
 }
 
 int32_t gs_b200_step_device_hook(int32_t V, int32_t H, int32_t W, int32_t sh_degree, float scale_modifier,
@@ -945,17 +909,12 @@ int32_t gs_b200_step_device_hook(int32_t V, int32_t H, int32_t W, int32_t sh_deg
                                  const float* means3D, const float* shs, const float* opacities, const float* scales,
                                  const float* rotations, float* dL_dout, float* grads, float* images, int32_t* radii,
                                  gs_b200_view_hook hook, void* hook_user, int64_t* num_rendered_out, void* stream_) {
-    cudaStream_t s = (cudaStream_t)stream_;
-    if (V <= 0 || N <= 0 || !views_host || !views_dev || !means3D || !shs || !opacities || !scales || !rotations ||
-        !dL_dout || !grads || !images || !hook) { gs_set_error("step_device_hook: bad argument"); return 1; }
-    PackedPtrs par; par.means = (float*)means3D; par.shs = (float*)shs; par.opac = (float*)opacities;
-    par.scales = (float*)scales; par.rots = (float*)rotations; par.m2d = nullptr;
-    const size_t n_grad = (size_t)N * (3 + 3 * (size_t)M + 1 + 3 + 4) + (size_t)N * 3;
-    (void)n_grad;   // grads need no memset: the first chunk's preprocess-backward writes every element
-    const PackedPtrs grd = carve_packed(grads, N, M, true);
+    GS_REQ(V > 0 && N > 0 && views_host && views_dev && means3D && shs && opacities && scales && rotations && dL_dout &&
+           grads && images && hook, "bad argument");
     StepOpts o; o.hook = hook; o.hook_user = hook_user; o.radii_out = radii;
-    return step_core(V, H, W, sh_degree, scale_modifier, views_host, views_dev, N, M, par, dL_dout, nullptr, grd, images,
-                     num_rendered_out, s, nullptr, &o);
+    return step_core(V, H, W, sh_degree, scale_modifier, views_host, views_dev, N, M,
+                     param_ptrs(means3D, shs, opacities, scales, rotations), dL_dout, nullptr,
+                     carve_packed(grads, N, M, true), images, num_rendered_out, (cudaStream_t)stream_, o);
 }
 
 namespace {
@@ -981,7 +940,7 @@ int32_t gs_b200_image_loss(int32_t H, int32_t W, const float* image, const float
                            float lambda_ssim, float lambda_alpha, float scale, float* dL_dimage, float* loss_out,
                            void* stream_) {
     cudaStream_t s = (cudaStream_t)stream_;
-    if (!image || !ref_image || !ref_mask || !dL_dimage || !loss_out) { gs_set_error("image_loss: NULL argument"); return 1; }
+    GS_REQ(image && ref_image && ref_mask && dL_dimage && loss_out, "NULL argument");
     if (Slot::ensure(g_loss_ws, gs_image_loss_scratch_bytes(H, W), s)) return 1;
     return gs_launch_image_loss(H, W, image, ref_image, ref_mask, lambda_ssim, lambda_alpha, scale, dL_dimage, loss_out,
                                 g_loss_ws.p, s);
@@ -993,19 +952,14 @@ int32_t gs_b200_step_device_train(int32_t V, int32_t H, int32_t W, int32_t sh_de
                                   const float* rotations, const float* ref_images, const float* ref_masks,
                                   float lambda_ssim, float lambda_alpha, float loss_scale, float* dL_dout, float* grads,
                                   float* images, int32_t* radii, float* losses, int64_t* num_rendered_out, void* stream_) {
-    cudaStream_t s = (cudaStream_t)stream_;
-    if (V <= 0 || N <= 0 || !views_host || !views_dev || !means3D || !shs || !opacities || !scales || !rotations ||
-        !ref_images || !ref_masks || !dL_dout || !grads || !images || !losses) { gs_set_error("step_device_train: bad argument"); return 1; }
-    if (lambda_ssim > 0.f && (H <= 160 || W <= 160)) { gs_set_error("step_device_train: MS-SSIM needs image sides > 160"); return 1; }
-    PackedPtrs par; par.means = (float*)means3D; par.shs = (float*)shs; par.opac = (float*)opacities;
-    par.scales = (float*)scales; par.rots = (float*)rotations; par.m2d = nullptr;
-    const size_t n_grad = (size_t)N * (3 + 3 * (size_t)M + 1 + 3 + 4) + (size_t)N * 3;
-    (void)n_grad;   // grads need no memset: the first chunk's preprocess-backward writes every element
-    const PackedPtrs grd = carve_packed(grads, N, M, true);
+    GS_REQ(V > 0 && N > 0 && views_host && views_dev && means3D && shs && opacities && scales && rotations &&
+           ref_images && ref_masks && dL_dout && grads && images && losses, "bad argument");
+    GS_REQ(!(lambda_ssim > 0.f) || (H > 160 && W > 160), "MS-SSIM needs image sides > 160");
     TrainLossCtx ctx{H, W, ref_images, ref_masks, lambda_ssim, lambda_alpha, loss_scale, dL_dout, images, losses};
     StepOpts o; o.hook = train_loss_hook; o.hook_user = &ctx; o.radii_out = radii;
-    return step_core(V, H, W, sh_degree, scale_modifier, views_host, views_dev, N, M, par, dL_dout, nullptr, grd, images,
-                     num_rendered_out, s, nullptr, &o);
+    return step_core(V, H, W, sh_degree, scale_modifier, views_host, views_dev, N, M,
+                     param_ptrs(means3D, shs, opacities, scales, rotations), dL_dout, nullptr,
+                     carve_packed(grads, N, M, true), images, num_rendered_out, (cudaStream_t)stream_, o);
 }
 
 int32_t gs_b200_render_views(int32_t V, int32_t H, int32_t W, int32_t sh_degree, float scale_modifier,
@@ -1013,25 +967,22 @@ int32_t gs_b200_render_views(int32_t V, int32_t H, int32_t W, int32_t sh_degree,
                              const float* means3D, const float* shs, const float* colors_precomp, const float* opacities,
                              const float* scales, const float* rotations, float* images, int32_t* radii,
                              int64_t* num_rendered_out, void* stream_) {
-    cudaStream_t s = (cudaStream_t)stream_;
-    if (V <= 0 || N <= 0 || !views_host || !views_dev || !means3D || !opacities || !scales || !rotations || !images) {
-        gs_set_error("render_views: bad argument"); return 1; }
+    GS_REQ(V > 0 && N > 0 && views_host && views_dev && means3D && opacities && scales && rotations && images,
+           "bad argument");
     if ((shs == nullptr) == (colors_precomp == nullptr)) { gs_set_error("Please provide excatly one of either SHs or precomputed colors!"); return 1; }
-    PackedPtrs par; par.means = (float*)means3D; par.shs = (float*)shs; par.colors = (float*)colors_precomp; par.opac = (float*)opacities;
-    par.scales = (float*)scales; par.rots = (float*)rotations; par.m2d = nullptr;
-    PackedPtrs grd{};
     StepOpts o; o.forward_only = true; o.radii_out = radii;
-    return step_core(V, H, W, sh_degree, scale_modifier, views_host, views_dev, N, M, par, nullptr, nullptr, grd, images,
-                     num_rendered_out, s, nullptr, &o);
+    return step_core(V, H, W, sh_degree, scale_modifier, views_host, views_dev, N, M,
+                     param_ptrs(means3D, shs, opacities, scales, rotations, colors_precomp), nullptr, nullptr,
+                     PackedPtrs{}, images, num_rendered_out, (cudaStream_t)stream_, o);
 }
 
-// ---- test entries of the binning stage ----------------------------------------------------------------------
+// ---- test entries of the binning stage and of the multi-view step's chunk stages ----------------------------------
 
 int32_t gs_b200_debug_sort_segmented(uint32_t* keys, uint32_t* keys_alt, uint32_t* vals, uint32_t* vals_alt,
                                      const int64_t* seg_off, int32_t nseg, int32_t begin_bit, int32_t end_bit,
                                      const uint32_t* key_bias, int32_t bias_stride, int32_t* result_in_alt, void* stream_) {
     cudaStream_t s = (cudaStream_t)stream_;
-    if (!seg_off || nseg < 1 || nseg > GS_MAX_SEGS || !result_in_alt) { gs_set_error("debug_sort_segmented: bad argument"); return 1; }
+    GS_REQ(seg_off && nseg >= 1 && nseg <= GS_MAX_SEGS && result_in_alt, "bad argument");
     SortSegs sg; sg.n = nseg;
     for (int i = 0; i <= nseg; i++) sg.off[i] = seg_off[i];
     void* scratch = nullptr;
@@ -1045,8 +996,9 @@ int32_t gs_b200_debug_sort_segmented(uint32_t* keys, uint32_t* keys_alt, uint32_
     return rc;
 }
 
-// The multi-view step's projection and binning, as step_core runs them (StepChunks, chunk_ws_setup, chunk_bin_a,
-// view_spans, chunk_bin_b), on `stream` alone, with every intermediate list copied out.
+// The multi-view step's projection and binning, as step_core runs them (chunk_project, chunk_bin), on `stream` alone,
+// with the pair buffers pre-filled with 0xFF bytes and every intermediate list copied out.  Without point_list (the
+// first call of two) only the [V][N] arrays and the totals, from which the caller sizes the pair lists.
 int32_t gs_b200_debug_bin_views(int32_t V, int32_t H, int32_t W, int32_t sh_degree, float scale_modifier,
                                 const float* views_dev, int32_t N, int32_t M, const float* means3D, const float* shs,
                                 const float* opacities, const float* scales, const float* rotations, int32_t tight,
@@ -1054,27 +1006,20 @@ int32_t gs_b200_debug_bin_views(int32_t V, int32_t H, int32_t W, int32_t sh_degr
                                 uint32_t* sorted_ids, uint32_t* offsets, int64_t* totals, uint32_t* ranges,
                                 uint32_t* point_list, uint32_t* tile_keys, void* stream_) {
     cudaStream_t s = (cudaStream_t)stream_;
-    if (V <= 0 || N <= 0 || M < (sh_degree + 1) * (sh_degree + 1) || M > 16 || !views_dev || !means3D || !shs ||
-        !opacities || !scales || !rotations || !radii || !tiles_touched || (tight && !spans) || !sorted_dkeys ||
-        !sorted_ids || !offsets || !totals || (point_list && (!tile_keys || !ranges))) {
-        gs_set_error("debug_bin_views: bad argument"); return 1;
-    }
-    struct Regions {
-        Region r[6];
-        ~Regions() { for (Region& x : r) if (x.p) cudaFree(x.p); }
-    } R;
-    const int tiles_x = (W + GS_TILE - 1) / GS_TILE, tiles_y = (H + GS_TILE - 1) / GS_TILE, ntiles = tiles_x * tiles_y;
-    const StepChunks ch(V);
+    GS_REQ(V > 0 && N > 0 && M >= (sh_degree + 1) * (sh_degree + 1) && M <= 16 && views_dev && means3D && shs &&
+           opacities && scales && rotations && radii && tiles_touched && (!tight || spans) && sorted_dkeys &&
+           sorted_ids && offsets && totals && (!point_list || (tile_keys && ranges)), "bad argument");
+    const StepScene sc(V, H, W, sh_degree, scale_modifier, views_dev, N, M,
+                       param_ptrs(means3D, shs, opacities, scales, rotations));
+    const int ntiles = sc.tiles_x * sc.tiles_y;
     ChunkWS w;
-    if (chunk_ws_setup(w, R.r[0], R.r[1], R.r[2], R.r[3], R.r[4], ch.VB, N, ntiles, tight != 0, s)) return 1;
-    PackedPtrs par; par.means = (float*)means3D; par.shs = (float*)shs; par.opac = (float*)opacities;
-    par.scales = (float*)scales; par.rots = (float*)rotations; par.m2d = nullptr;
+    if (w.setup(sc, tight != 0, s)) return 1;
     unsigned long long host_totals[GS_MAX_SEGS];
     int64_t pair0 = 0;        // the chunk's first pair in point_list / tile_keys
-    for (int k = 0; k < ch.nchunks; k++) {
-        const int v0 = k * ch.VB, nv = std::min(ch.VB, V - v0);
+    for (int k = 0; k < sc.ch.nchunks; k++) {
+        const int v0 = sc.ch.first(k), nv = sc.ch.count(k);
         const size_t o = (size_t)v0 * N, n = (size_t)nv * N;
-        if (chunk_bin_a(w, views_dev + (size_t)v0 * 40, nv, W, H, sh_degree, scale_modifier, N, M, par, 0, host_totals, s)) return 1;
+        if (chunk_project(w, sc, k, host_totals, s)) return 1;
         GS_CUDA_CHECK(cudaMemcpyAsync(radii + o, w.radii, n * 4, cudaMemcpyDeviceToDevice, s));
         GS_CUDA_CHECK(cudaMemcpyAsync(tiles_touched + o, w.bin.tiles, n * 4, cudaMemcpyDeviceToDevice, s));
         if (tight) GS_CUDA_CHECK(cudaMemcpyAsync(spans + 4 * o, w.spans, n * 16, cudaMemcpyDeviceToDevice, s));
@@ -1083,59 +1028,64 @@ int32_t gs_b200_debug_bin_views(int32_t V, int32_t H, int32_t W, int32_t sh_degr
         GS_CUDA_CHECK(cudaMemcpyAsync(offsets + o, w.bin.offsets, n * 4, cudaMemcpyDeviceToDevice, s));
         GS_CUDA_CHECK(cudaStreamSynchronize(s));
         for (int j = 0; j < nv; j++) totals[v0 + j] = (int64_t)host_totals[j];
-        ViewSpans vs;
-        if (view_spans(nv, host_totals, vs)) return 1;
-        if (!point_list) continue;      // first call of two: the caller sizes the pair lists from `totals`
-        const int64_t P = vs.base[nv];
-        if (Slot::ensure(R.r[5], chunk_pairs_bytes(nv, P), s)) return 1;
-        // a pair slot the emit leaves unwritten keeps this value through the sort
-        GS_CUDA_CHECK(cudaMemsetAsync(R.r[5].p, 0xFF, chunk_pairs_bytes(nv, P), s));
-        BinB b;
-        if (chunk_bin_b(w, vs, R.r[5].p, b, tiles_x, tiles_y, s)) return 1;
-        GS_CUDA_CHECK(cudaMemcpyAsync(ranges + (size_t)v0 * ntiles * 2, w.ranges, (size_t)nv * ntiles * 8, cudaMemcpyDeviceToDevice, s));
-        if (P > 0) {
-            GS_CUDA_CHECK(cudaMemcpyAsync(point_list + pair0, b.point_list, (size_t)P * 4, cudaMemcpyDeviceToDevice, s));
-            GS_CUDA_CHECK(cudaMemcpyAsync(tile_keys + pair0, b.tile_keys, (size_t)P * 4, cudaMemcpyDeviceToDevice, s));
+        if (chunk_bin(w, sc, k, host_totals, true, s)) return 1;
+        if (point_list) {
+            const int64_t P = w.vs.base[nv];
+            GS_CUDA_CHECK(cudaMemcpyAsync(ranges + (size_t)v0 * ntiles * 2, w.ranges, (size_t)nv * ntiles * 8, cudaMemcpyDeviceToDevice, s));
+            if (P > 0) {
+                GS_CUDA_CHECK(cudaMemcpyAsync(point_list + pair0, w.pairs.point_list, (size_t)P * 4, cudaMemcpyDeviceToDevice, s));
+                GS_CUDA_CHECK(cudaMemcpyAsync(tile_keys + pair0, w.pairs.tile_keys, (size_t)P * 4, cudaMemcpyDeviceToDevice, s));
+            }
+            pair0 += P;
         }
-        pair0 += P;
         GS_CUDA_CHECK(cudaStreamSynchronize(s));
     }
     return 0;
 }
 
-// The multi-view step's batched preprocess, as step_core runs it (StepChunks, chunk_ws_setup, chunk_bin_a; with
-// geom_only the host-buffer step's colour-free pass, then gs_launch_sh_colour_multi), with the records copied out.
+// The multi-view step's batched preprocess, as step_core runs it (chunk_project, chunk_bin; with geom_only the
+// host-buffer step's colour-free projection and the colour pass after the binning), with the records copied out.
 int32_t gs_b200_debug_preprocess_views(int32_t V, int32_t H, int32_t W, int32_t sh_degree, float scale_modifier,
                                        const float* views_dev, int32_t N, int32_t M, const float* means3D,
                                        const float* shs, const float* colors_precomp, const float* opacities,
                                        const float* scales, const float* rotations, int32_t geom_only, float* recs_out,
                                        void* stream_) {
     cudaStream_t s = (cudaStream_t)stream_;
-    if (V <= 0 || N <= 0 || sh_degree < 0 || sh_degree > 3 || !views_dev || !means3D || !opacities || !scales ||
-        !rotations || !recs_out || (shs == nullptr) == (colors_precomp == nullptr) || (geom_only && !shs) ||
-        (shs && (M < (sh_degree + 1) * (sh_degree + 1) || M > 16))) {
-        gs_set_error("debug_preprocess_views: bad argument"); return 1;
-    }
-    struct Regions {
-        Region r[5];
-        ~Regions() { for (Region& x : r) if (x.p) cudaFree(x.p); }
-    } R;
-    const int tiles_x = (W + GS_TILE - 1) / GS_TILE, tiles_y = (H + GS_TILE - 1) / GS_TILE;
-    const StepChunks ch(V);
+    GS_REQ(V > 0 && N > 0 && sh_degree >= 0 && sh_degree <= 3 && views_dev && means3D && opacities && scales &&
+           rotations && recs_out && (shs == nullptr) != (colors_precomp == nullptr) && (!geom_only || shs) &&
+           (!shs || (M >= (sh_degree + 1) * (sh_degree + 1) && M <= 16)), "bad argument");
+    const StepScene sc(V, H, W, sh_degree, scale_modifier, views_dev, N, M,
+                       param_ptrs(means3D, shs, opacities, scales, rotations, colors_precomp), geom_only != 0);
     ChunkWS w;
-    if (chunk_ws_setup(w, R.r[0], R.r[1], R.r[2], R.r[3], R.r[4], ch.VB, N, tiles_x * tiles_y,
-                       g_tile_culling.load() >= 1, s)) return 1;
-    PackedPtrs par; par.means = (float*)means3D; par.shs = (float*)shs; par.colors = (float*)colors_precomp;
-    par.opac = (float*)opacities; par.scales = (float*)scales; par.rots = (float*)rotations; par.m2d = nullptr;
+    if (w.setup(sc, g_tile_culling.load() >= 1, s)) return 1;
     unsigned long long host_totals[GS_MAX_SEGS];
-    for (int k = 0; k < ch.nchunks; k++) {
-        const int v0 = k * ch.VB, nv = std::min(ch.VB, V - v0);
-        const float* vchunk = views_dev + (size_t)v0 * 40;
-        if (chunk_bin_a(w, vchunk, nv, W, H, sh_degree, scale_modifier, N, M, par, geom_only ? 1 : 0, host_totals, s)) return 1;
-        if (geom_only && gs_launch_sh_colour_multi(vchunk, nv, sh_degree, N, M, par.means, par.shs, w.radii, w.recs, s)) return 1;
-        GS_CUDA_CHECK(cudaMemcpyAsync(recs_out + (size_t)v0 * N * 12, w.recs, (size_t)nv * N * sizeof(SplatRec),
-                                      cudaMemcpyDeviceToDevice, s));
+    for (int k = 0; k < sc.ch.nchunks; k++) {
+        if (chunk_project(w, sc, k, host_totals, s)) return 1;
         GS_CUDA_CHECK(cudaStreamSynchronize(s));
+        if (chunk_bin(w, sc, k, host_totals, false, s)) return 1;
+        GS_CUDA_CHECK(cudaMemcpyAsync(recs_out + (size_t)sc.ch.first(k) * N * 12, w.recs,
+                                      (size_t)sc.ch.count(k) * N * sizeof(SplatRec), cudaMemcpyDeviceToDevice, s));
+        GS_CUDA_CHECK(cudaStreamSynchronize(s));
+    }
+    return 0;
+}
+
+// The preprocess backward of the multi-view step, as step_core runs it (chunk_backward), from the caller's [V][N]
+// radii and SplatGrad; the last chunk over `nparts` Gaussian ranges as with a gradient sink.
+int32_t gs_b200_debug_preprocess_backward_multi(int32_t V, int32_t H, int32_t W, int32_t sh_degree, float scale_modifier,
+                                                const float* views_dev, int32_t N, int32_t M, const float* means3D,
+                                                const float* shs, const float* scales, const float* rotations,
+                                                const int32_t* radii, const double* splat_grads, float* grads_dev,
+                                                int32_t nparts, void* stream_) {
+    GS_REQ(V > 0 && N > 0 && M >= (sh_degree + 1) * (sh_degree + 1) && M <= 16 && nparts >= 1 && views_dev &&
+           means3D && shs && scales && rotations && radii && splat_grads && grads_dev, "bad argument");
+    const StepScene sc(V, H, W, sh_degree, scale_modifier, views_dev, N, M,
+                       param_ptrs(means3D, shs, nullptr, scales, rotations));
+    const PackedPtrs grd = carve_packed(grads_dev, N, M, true);
+    for (int k = 0; k < sc.ch.nchunks; k++) {
+        const size_t o = (size_t)sc.ch.first(k) * N;
+        if (chunk_backward(sc, k, radii + o, (const SplatGrad*)splat_grads + o, grd, k + 1 == sc.ch.nchunks ? nparts : 1,
+                           nullptr, (cudaStream_t)stream_)) return 1;
     }
     return 0;
 }
@@ -1145,7 +1095,7 @@ int32_t gs_b200_step_host(int32_t V, int32_t H, int32_t W, int32_t sh_degree, fl
                           const float* shs_host, const float* opacities_host, const float* scales_host,
                           const float* rotations_host, const float* dL_dout_host, float* grads_host,
                           float* images_host, int64_t* num_rendered_out, void* stream_) {
-    return step_host_impl(V, H, W, sh_degree, scale_modifier, views_host, N, M, means3D_host, shs_host,
+    return step_host_impl(__func__, V, H, W, sh_degree, scale_modifier, views_host, N, M, means3D_host, shs_host,
                           opacities_host, scales_host, rotations_host, dL_dout_host, grads_host, nullptr,
                           images_host, num_rendered_out, stream_);
 }
@@ -1155,7 +1105,7 @@ int32_t gs_b200_step_host_dev_grads(int32_t V, int32_t H, int32_t W, int32_t sh_
                           const float* shs_host, const float* opacities_host, const float* scales_host,
                           const float* rotations_host, const float* dL_dout_host, float* grads_dev,
                           float* images_host, int64_t* num_rendered_out, void* stream_) {
-    return step_host_impl(V, H, W, sh_degree, scale_modifier, views_host, N, M, means3D_host, shs_host,
+    return step_host_impl(__func__, V, H, W, sh_degree, scale_modifier, views_host, N, M, means3D_host, shs_host,
                           opacities_host, scales_host, rotations_host, dL_dout_host, nullptr, grads_dev,
                           images_host, num_rendered_out, stream_);
 }

@@ -168,6 +168,44 @@ def test_dr_and_ngp_entry_points_refuse_bad_arguments_with_their_messages():
     assert lib.ngp_b200_mlp2_supported(24, 32, 1) == 1 and lib.ngp_b200_mlp2_supported(16, 32, 1) == 0
 
 
+def test_rasterizer_entry_points_refuse_bad_arguments_with_their_messages():
+    """Every argument-taking gs_b200_* entry point of the rasterizer and the multi-view step, called with arguments
+    that fail its first check, returns 1 (gs_b200_step_view_chunks: -1) and sets gs_b200_last_error() to exactly
+    "<entry point>: <message>", before any CUDA call: without a GPU, one would set a CUDA error instead."""
+    from gs_b200 import _lib
+    lib = _lib.lib
+
+    def call(name, *lead):               # the given leading arguments, then zero / NULL for all the others
+        fn = getattr(lib, name)
+        return fn(*lead, *(t() for t in fn.argtypes[len(lead):]))
+
+    sink = _lib.GRAD_SINK(lambda user, first, count, stream: None)
+    refused = {      # name: (leading arguments, message); V = 0 fails every step entry first
+        "gs_b200_set_tile_culling": ((3,), "tile culling mode must be 0, 1 or 2"),
+        "gs_b200_rasterize_forward": ((), "NULL view field"),
+        "gs_b200_rasterize_backward": ((), "NULL view field"),
+        "gs_b200_debug_sorted_keys": ((), "NULL argument"),
+        "gs_b200_debug_preprocess_backward": ((), "NULL view field"),
+        "gs_b200_debug_preprocess_backward_multi": ((), "bad argument"),
+        "gs_b200_set_grad_sink": ((sink,), "nchunks must be 1..64"),
+        "gs_b200_step_device": ((), "bad argument"),
+        "gs_b200_step_device_hook": ((), "bad argument"),
+        "gs_b200_image_loss": ((), "NULL argument"),
+        "gs_b200_step_device_train": ((), "bad argument"),
+        "gs_b200_render_views": ((), "bad argument"),
+        "gs_b200_debug_sort_segmented": ((), "bad argument"),
+        "gs_b200_debug_bin_views": ((), "bad argument"),
+        "gs_b200_debug_preprocess_views": ((), "bad argument"),
+        "gs_b200_step_host": ((), "bad argument"),
+        "gs_b200_step_host_dev_grads": ((), "bad argument"),
+    }
+    for name, (lead, msg) in refused.items():
+        assert call(name, *lead) == 1, name
+        assert _lib.last_error() == f"{name}: {msg}"
+    assert call("gs_b200_step_view_chunks") == -1
+    assert _lib.last_error() == "gs_b200_step_view_chunks: bad argument"
+
+
 def test_settings_namedtuple_field_order_matches_reference_call_site():
     # main_3DGS_renderer.py:849-862 constructs it by keyword; LGM/TRELLIS too. Order = the package's NamedTuple.
     from diff_gaussian_rasterization import GaussianRasterizationSettings
